@@ -215,7 +215,7 @@ int b200conv_ir_decay_eq(int device, float* ir, size_t n, const double* lut, dou
 /* SURVEY 8f-3, the pipeline: the device-resident subset of Impulse::recalcImpulse (src/dsp/Impulse.cpp:297-360) in the
  * reference's order — auto gain (:313-320, :703-720), reverse (:322-330), trim (:437-470), gain (:472-486), decay EQ
  * (:602-648), clip (:488-501), attack / decay envelope (:651-680) — on the raw taps of all 2 / 4 channels with ONE upload.
- * (Resampling, stretch and the parametric EQ stay on the host.)
+ * (No resampling, stretch or parametric EQ, and a ready-made decay table: b200conv_ir_recalc below adds those.)
  *   b200conv_ir_shape            shaped taps back to the host (out[c] needs room for n floats, *out_len taps written);
  *   b200conv_init_*_shaped       shape on the device and build the partition spectra straight from the device-resident
  *                                taps — the IR never returns to the host between shaping and FFTConvolver::init. */
@@ -234,6 +234,40 @@ int b200conv_init_uniform_shaped(b200conv_t* h, size_t block, const float* const
                                  const b200conv_ir_shape_params* sp);
 int b200conv_init_twostage_shaped(b200conv_t* h, size_t head_block, size_t tail_block, const float* const* raw, size_t n,
                                   const b200conv_ir_shape_params* sp);
+
+/* SURVEY 8f-3, the whole of Impulse::recalcImpulse (src/dsp/Impulse.cpp:299-360) on the device, in the reference's order:
+ * auto gain -> reverse -> resampling to the project rate (:362-389) -> stretch (:391-434) -> trim -> gain -> parametric EQ
+ * (:503-537) -> decay EQ (:539-599, the 2049-entry table is built from the bands inside) -> clip -> envelope.
+ * Resampling and stretch follow JUCE's ResamplingAudioSource (linear interpolation, second-order low pass in double
+ * precision before down-sampling / after up-sampling); the EQ bands are REEV-R's SVF sections (src/dsp/SVF.cpp), with
+ * Off and unknown modes run as a peak band, as Impulse.cpp:511-519 does.  Channel order {LL, RR[, LR, RL]}; one upload.
+ *   b200conv_ir_recalc_len     output taps per channel (host arithmetic only; 0 if p is NULL); can exceed n
+ *                              (up-sampling and positive stretch);
+ *   b200conv_ir_recalc         taps back to the host: out[c] has room for out_cap >= b200conv_ir_recalc_len(n, p) floats;
+ *   b200conv_init_*_recalc     recalculate and build the partition spectra from the device-resident taps (no download).
+ * B200CONV_EINVAL: a NULL pointer, srate or ir_srate <= 0, more than 8 bands or a mode outside 0..9, out_cap too small. */
+typedef struct b200conv_eq_band {
+  int mode;                         /* SVF::Mode: 0 LP, 1 BP, 2 HP, 3 LS, 4 HS, 5 PK, 6 BS, 7 HP6, 8 LP6, 9 Off */
+  float freq, q, gain;
+} b200conv_eq_band;
+typedef struct b200conv_ir_recalc_params {
+  double ir_srate, srate;           /* rate of the IR file / of the session (Impulse::irsrate / srate)               */
+  float stretch;                    /* Impulse::stretch (-1..1 in REEV-R): rate factor 2^stretch                       */
+  int autogain, reverse;
+  float trim_left, trim_right, gain;
+  int n_param_eq; const b200conv_eq_band* param_eq;   /* applyParamEQ, <= 8 bands (0: off)                        */
+  int n_decay_eq; const b200conv_eq_band* decay_eq;   /* applyDecayEQ, <= 8 bands (0: off)                        */
+  float decay_rate;                 /* Impulse::decayRate                                                              */
+  int clip;
+  float attack, decay;              /* fractions of the (trimmed) length                                               */
+} b200conv_ir_recalc_params;
+size_t b200conv_ir_recalc_len(size_t n, const b200conv_ir_recalc_params* p);
+int b200conv_ir_recalc(int device, const float* const* raw, int n_channels, size_t n, const b200conv_ir_recalc_params* p,
+                       float* const* out, size_t out_cap, size_t* out_len);
+int b200conv_init_uniform_recalc(b200conv_t* h, size_t block, const float* const* raw, size_t n,
+                                 const b200conv_ir_recalc_params* p);
+int b200conv_init_twostage_recalc(b200conv_t* h, size_t head_block, size_t tail_block, const float* const* raw, size_t n,
+                                  const b200conv_ir_recalc_params* p);
 
 /* Pinned host memory helpers (staging buffers for the e2e path).  register/unregister page-lock memory the caller
  * owns (e.g. a shared-memory region several per-GPU processes write their output slices into). */

@@ -37,6 +37,19 @@ class IrShapeParams(C.Structure):
                 ("attack", C.c_float), ("decay", C.c_float)]
 
 
+class EqBand(C.Structure):
+    """b200conv_eq_band: one SVF band (mode 0..9 = LP BP HP LS HS PK BS HP6 LP6 Off)."""
+    _fields_ = [("mode", C.c_int), ("freq", C.c_float), ("q", C.c_float), ("gain", C.c_float)]
+
+
+class IrRecalcParams(C.Structure):
+    _fields_ = [("ir_srate", C.c_double), ("srate", C.c_double), ("stretch", C.c_float), ("autogain", C.c_int),
+                ("reverse", C.c_int), ("trim_left", C.c_float), ("trim_right", C.c_float), ("gain", C.c_float),
+                ("n_param_eq", C.c_int), ("param_eq", C.POINTER(EqBand)), ("n_decay_eq", C.c_int),
+                ("decay_eq", C.POINTER(EqBand)), ("decay_rate", C.c_float), ("clip", C.c_int), ("attack", C.c_float),
+                ("decay", C.c_float)]
+
+
 class StageInfo(C.Structure):
     _fields_ = [
         ("block", C.c_size_t),
@@ -93,6 +106,10 @@ SYMBOLS = [
     ("b200conv_ir_shape", C.c_int, [C.c_int, _PP, C.c_int, C.c_size_t, C.c_void_p, _PP, C.c_void_p]),
     ("b200conv_init_uniform_shaped", C.c_int, [C.c_void_p, C.c_size_t, _PP, C.c_size_t, C.c_void_p]),
     ("b200conv_init_twostage_shaped", C.c_int, [C.c_void_p, C.c_size_t, C.c_size_t, _PP, C.c_size_t, C.c_void_p]),
+    ("b200conv_ir_recalc_len", C.c_size_t, [C.c_size_t, C.c_void_p]),
+    ("b200conv_ir_recalc", C.c_int, [C.c_int, _PP, C.c_int, C.c_size_t, C.c_void_p, _PP, C.c_size_t, C.c_void_p]),
+    ("b200conv_init_uniform_recalc", C.c_int, [C.c_void_p, C.c_size_t, _PP, C.c_size_t, C.c_void_p]),
+    ("b200conv_init_twostage_recalc", C.c_int, [C.c_void_p, C.c_size_t, C.c_size_t, _PP, C.c_size_t, C.c_void_p]),
     ("b200conv_alloc_host", C.c_void_p, [C.c_size_t]),
     ("b200conv_free_host", None, [C.c_void_p]),
     ("b200conv_version", C.c_char_p, []),

@@ -87,6 +87,36 @@ class Engine:
         return self._check(self._l.b200conv_init_uniform_shaped(self._h, block, ptrs, keep[0].size, C.byref(sp)),
                            "init_uniform_shaped", True) == 0
 
+    @staticmethod
+    def _recalc_params(ir_srate=48000.0, srate=48000.0, stretch=0.0, autogain=True, reverse=False, trim_left=0.0,
+                       trim_right=0.0, gain=1.0, param_eq=(), decay_eq=(), decay_rate=1.0, clip=True, attack=0.0, decay=0.0):
+        """b200conv_ir_recalc_params; bands: (mode, freq, q, gain) tuples (mode = SVF::Mode 0..9).  Returns the struct and
+        the band arrays it points to (keep them alive for the call)."""
+        def bands(bs):
+            bs = list(bs or [])
+            arr = (_lib.EqBand * max(len(bs), 1))(*[_lib.EqBand(int(m), f, q, g) for m, f, q, g in bs])
+            return len(bs), arr
+        npq, pq = bands(param_eq)
+        ndc, dc = bands(decay_eq)
+        rp = _lib.IrRecalcParams(float(ir_srate), float(srate), stretch, int(autogain), int(reverse), trim_left, trim_right,
+                                 gain, npq, C.cast(pq, C.POINTER(_lib.EqBand)), ndc, C.cast(dc, C.POINTER(_lib.EqBand)),
+                                 decay_rate, int(clip), attack, decay)
+        return rp, (pq, dc)
+
+    def init_twostage_recalc(self, head: int, tail: int, raw_irs, **recalc) -> bool:
+        """The whole Impulse::recalcImpulse on the device (resampling, stretch, parametric and decay EQ included), partition
+        spectra built from the device-resident taps (b200conv_init_twostage_recalc); raw_irs: equally long raw channels."""
+        keep, ptrs, lens = self._irs(raw_irs)
+        rp, bands = self._recalc_params(**recalc)
+        return self._check(self._l.b200conv_init_twostage_recalc(self._h, head, tail, ptrs, keep[0].size, C.byref(rp)),
+                           "init_twostage_recalc", True) == 0
+
+    def init_uniform_recalc(self, block: int, raw_irs, **recalc) -> bool:
+        keep, ptrs, lens = self._irs(raw_irs)
+        rp, bands = self._recalc_params(**recalc)
+        return self._check(self._l.b200conv_init_uniform_recalc(self._h, block, ptrs, keep[0].size, C.byref(rp)),
+                           "init_uniform_recalc", True) == 0
+
     def init_stages(self, blocks, offsets, irs) -> bool:
         keep, ptrs, lens = self._irs(irs)
         b = (C.c_size_t * len(blocks))(*blocks)
@@ -314,6 +344,32 @@ def ir_shape(raw_irs, device: int = 0, lib=None, **shape):
     rc = lib.b200conv_ir_shape(device, _ptr_array(raws), len(raws), n, C.byref(sp), _ptr_array(outs), C.byref(m))
     if rc != 0:
         raise B200ConvError(f"b200conv_ir_shape failed ({rc})")
+    return [o[:m.value].copy() for o in outs]
+
+
+def ir_recalc_len(n: int, lib=None, **recalc) -> int:
+    """Taps per channel that ir_recalc returns for n raw taps (b200conv_ir_recalc_len)."""
+    lib = lib or _lib.default()
+    rp, bands = Engine._recalc_params(**recalc)
+    return int(lib.b200conv_ir_recalc_len(n, C.byref(rp)))
+
+
+def ir_recalc(raw_irs, device: int = 0, lib=None, **recalc):
+    """Device version of the whole Impulse::recalcImpulse (b200conv_ir_recalc); raw_irs = {LL, RR[, LR, RL]}, equally long.
+    Keywords: ir_srate, srate, stretch, autogain, reverse, trim_left, trim_right, gain, param_eq, decay_eq (lists of
+    (mode, freq, q, gain)), decay_rate, clip, attack, decay.  Returns the recalculated channels."""
+    lib = lib or _lib.default()
+    raws = [np.ascontiguousarray(a, dtype=np.float32) for a in raw_irs]
+    n = raws[0].size
+    if any(a.size != n for a in raws):
+        raise ValueError("raw channels must be equally long")
+    rp, bands = Engine._recalc_params(**recalc)
+    cap = int(lib.b200conv_ir_recalc_len(n, C.byref(rp)))
+    outs = [np.empty(max(cap, 1), np.float32) for _ in raws]
+    m = C.c_size_t(0)
+    rc = lib.b200conv_ir_recalc(device, _ptr_array(raws), len(raws), n, C.byref(rp), _ptr_array(outs), cap, C.byref(m))
+    if rc != 0:
+        raise B200ConvError(f"b200conv_ir_recalc failed ({rc})")
     return [o[:m.value].copy() for o in outs]
 
 

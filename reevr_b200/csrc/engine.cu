@@ -1864,18 +1864,23 @@ int b200conv_init_stages(b200conv_t* h, int n_stages, const size_t* blocks, cons
   return init_common(h, n_stages, blocks, offsets, ir, ir_len);
 }
 
-// irshape.cu (internal): shape raw host taps into device buffers
+// irshape.cu (internal): shape / recalculate raw host taps into device buffers
 int pc_ir_shape_to_device(int device, const float* const* raw, int C, size_t n, const b200conv_ir_shape_params* sp,
                           float** dev_out, size_t* out_len, size_t* trimmed);
+int pc_ir_recalc_to_device(int device, const float* const* raw, int C, size_t n, const b200conv_ir_recalc_params* p,
+                           float** dev_out, size_t* out_len, size_t* trimmed);
 void pc_ir_shape_free(float** dev_out, int C);
 
+// exactly one of sp (b200conv_init_*_shaped) and rp (b200conv_init_*_recalc) is set
 static int init_shaped(b200conv_t* h, int n_stages, const size_t* blocks, const size_t* offsets,
-                       const float* const* raw, size_t n, const b200conv_ir_shape_params* sp) {
-  if (!raw || !sp) return fail(h, B200CONV_EINVAL, "null argument");
+                       const float* const* raw, size_t n, const b200conv_ir_shape_params* sp,
+                       const b200conv_ir_recalc_params* rp = nullptr) {
+  if (!raw || (!sp && !rp)) return fail(h, B200CONV_EINVAL, "null argument");
   if (h->C < 2 || h->C > 8) return fail(h, B200CONV_ESTATE, "IR shaping works on 2..8 channel handles (LL, RR[, LR, RL])");
   float* dev[8] = {};
   size_t m = 0, trimmed[8] = {}, lens[8] = {};
-  if (int rc = pc_ir_shape_to_device(h->cfg.device, raw, h->C, n, sp, dev, &m, trimmed))
+  if (int rc = sp ? pc_ir_shape_to_device(h->cfg.device, raw, h->C, n, sp, dev, &m, trimmed)
+                  : pc_ir_recalc_to_device(h->cfg.device, raw, h->C, n, rp, dev, &m, trimmed))
     return fail(h, rc, "IR shaping on the device failed");
   for (int c = 0; c < h->C; ++c) lens[c] = m;
   h->ir_on_device = true; h->ir_trimmed = trimmed;
@@ -1900,6 +1905,23 @@ int b200conv_init_twostage_shaped(b200conv_t* h, size_t head_block, size_t tail_
   const size_t blocks[2] = {hb, tb};
   const size_t offsets[2] = {0, 2 * tb};
   return init_shaped(h, 2, blocks, offsets, raw, n, sp);
+}
+
+int b200conv_init_uniform_recalc(b200conv_t* h, size_t block, const float* const* raw, size_t n, const b200conv_ir_recalc_params* p) {
+  REQUIRE_CUDA(h);
+  const size_t off = 0;
+  return init_shaped(h, 1, &block, &off, raw, n, nullptr, p);
+}
+
+int b200conv_init_twostage_recalc(b200conv_t* h, size_t head_block, size_t tail_block, const float* const* raw, size_t n,
+                                  const b200conv_ir_recalc_params* p) {
+  REQUIRE_CUDA(h);
+  if (head_block == 0 || tail_block == 0) return fail(h, B200CONV_EINVAL, "block size 0");
+  if (head_block > tail_block) std::swap(head_block, tail_block);
+  const size_t hb = next_pow2(head_block), tb = next_pow2(tail_block);
+  const size_t blocks[2] = {hb, tb};
+  const size_t offsets[2] = {0, 2 * tb};
+  return init_shaped(h, 2, blocks, offsets, raw, n, nullptr, p);
 }
 
 int b200conv_process_device(b200conv_t* h, const float* in_dev, size_t in_stride,
