@@ -172,6 +172,24 @@ int b200conv_chain_configure(b200conv_t* h, const b200conv_chain_config* cfg);
 int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* ysend, const float* yrev,
                            float* const* out, size_t len);
 
+/* IR hot-swap inside the device chain (src/PluginProcessor.cpp:1655-1668, 1694-1756, 1799-1830).
+ * `live` has the chain configured; `incoming` holds the new IR (e.g. b200conv_init_twostage_recalc).
+ * The next b200conv_chain_process(live, ...) does the warm-up (0.25 s of send history, replayed on the device in
+ * ONE batched call, host_block = the host's samplesPerBlock), then the calls crossfade for ceil(srate * 0.05)
+ * samples. At the end of the call where the fade completes, the chain (filter states, predelay / warmer ring,
+ * configuration, staging) moves to `incoming`, and `live` no longer has a chain. The caller then swaps its
+ * pointers, exactly like std::swap(loadConvolver, convolver).
+ * The handles may differ in channel count (stereo <-> quad).  B200CONV_ESTATE: `live` has no chain, `incoming` has no
+ * IR or already owns a chain, or a swap is pending on either; while a swap is pending, b200conv_chain_configure on
+ * either handle and any init on either handle fail with B200CONV_ESTATE too.  B200CONV_EINVAL: the same handle twice,
+ * different devices, sharded or routed handles, unequal staging sizes, host_block == 0.  b200conv_reset /
+ * b200conv_destroy of either handle cancels the swap (the live handle continues alone); b200conv_clear(live) clears
+ * the chain's history as usual and leaves `incoming` as it is. */
+int b200conv_chain_swap(b200conv_t* live, b200conv_t* incoming, size_t host_block);
+/* 0 = no swap pending, 1 = armed (warm-up at the next chain call), 2 = fading,
+ * 3 = completed: this handle gave its chain away.                  */
+int b200conv_chain_swap_state(const b200conv_t* h);
+
 /* IR hot-swap helpers (SURVEY 8f-2; the reference replays a 0.25 s "warmer" ring through the freshly
  * loaded convolver call by call and crossfades two convolvers on the host for 50 ms,
  * src/PluginProcessor.cpp:1695-1750,1800-1830).

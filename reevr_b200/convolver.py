@@ -199,6 +199,16 @@ class Engine:
                 env[1].ctypes.data if env[1] is not None else None, _ptr_array(ys), n), "chain_process")
         return ys[0], ys[1]
 
+    def chain_swap(self, incoming: "Engine", host_block: int) -> None:
+        """IR hot swap inside the chain (b200conv_chain_swap): the next chain_process call replays the send history
+        through `incoming` and starts the 50 ms crossfade; when chain_swap_state() becomes 3 the chain has moved to
+        `incoming`, which the caller uses from then on (std::swap(loadConvolver, convolver))."""
+        self._check(self._l.b200conv_chain_swap(self._h, incoming._h, host_block), "chain_swap")
+
+    def chain_swap_state(self) -> int:
+        """0 no swap pending, 1 armed, 2 fading, 3 this handle gave its chain away."""
+        return int(self._l.b200conv_chain_swap_state(self._h))
+
     def clear(self):
         self._check(self._l.b200conv_clear(self._h), "clear")
 

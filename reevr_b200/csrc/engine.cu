@@ -154,13 +154,20 @@ struct b200conv {
   pc::ChainFilter chain_lc{}, chain_hc{};
   float* c_io = nullptr;             // [dry L, dry R, ysend, yrev, out L, out R][Lmax] staging
   float* c_conv_in = nullptr;        // [2][Lmax] convolver input (after filters + predelay)
-  float* c_filt = nullptr;           // [2][Lmax]
-  float* c_state = nullptr;          // [2][8] filter states
+  float* c_filt = nullptr;           // [3][Lmax]: filtered send of the call ; row 2 stays zero (LR / RL input of a
+                                     // quad handle being crossfaded in)
+  float* c_state = nullptr;          // [4][8] filter states: rows 0-1 the send, rows 2-3 the warm-up replay of a swap
   float* c_hpin = nullptr;           // pinned [dry L, dry R, ysend, yrev, out L, out R][hpin_cap]: zero-copy I/O of real-time chain calls
   float* c_hpin_dev = nullptr;
-  float* c_ring = nullptr;           // [2][ring] predelay ring
+  float* c_ring = nullptr;           // [2][ring] predelay ring; also the warmer of an IR hot swap (>= W samples of history)
   size_t c_ring_size = 0;
   long long c_ring_pos = 0;
+  // IR hot swap inside the chain (b200conv_chain_swap): swap_peer links the two handles of a pending swap
+  b200conv* swap_peer = nullptr;
+  int swap_state = 0;                // 0 none, 1 armed, 2 fading, 3 this handle gave its chain away
+  bool swap_live = false;            // the live side of the pending swap (holds the fade state below)
+  size_t swap_block = 0;             // host block of the warm-up replay
+  long long swap_xfade = 0, swap_xfadelen = 0;   // the reference's xfade / xfadelen counters
   // b200conv_init_*_shaped: the taps handed to init are DEVICE buffers (shaped there) with known post-trim lengths
   bool ir_on_device = false;
   const size_t* ir_trimmed = nullptr;
@@ -286,6 +293,7 @@ void free_all(b200conv* h) {
   h->c_io = h->c_conv_in = h->c_filt = h->c_state = h->c_ring = nullptr;
   h->c_ring_size = 0; h->c_ring_pos = 0;
   h->chain_on = false; h->route_in_only = false;
+  if (h->swap_state == 3) h->swap_state = 0;
   if (h->hpin_in) cudaFreeHost(h->hpin_in);
   if (h->hpin_out) cudaFreeHost(h->hpin_out);
   if (h->hflag) cudaFreeHost(h->hflag);
@@ -1057,6 +1065,7 @@ int init_impl(b200conv* h, int n_stages, const size_t* blocks, const size_t* off
 // nothing half-allocated, later init / process calls work.
 int init_common(b200conv* h, int n_stages, const size_t* blocks, const size_t* offsets,
                 const float* const* ir, const size_t* ir_len) {
+  if (h->swap_peer) return fail(h, B200CONV_ESTATE, "an IR hot swap is pending on this handle");
   const int rc = init_impl(h, n_stages, blocks, offsets, ir, ir_len);
   if (rc != B200CONV_OK && !h->sticky_cuda_error) {
     const std::string keep = h->err;
@@ -1709,6 +1718,14 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
   return 0;
 }
 
+// b200conv_reset / b200conv_destroy of either handle of a pending IR hot swap: the live handle continues alone
+void swap_cancel(b200conv* h) {
+  if (!h->swap_peer) return;
+  b200conv* p = h->swap_peer;
+  p->swap_peer = nullptr; p->swap_state = 0; p->swap_live = false;
+  h->swap_peer = nullptr; h->swap_state = 0; h->swap_live = false;
+}
+
 // make s_main wait for everything queued on s_post (end of an overlapped call)
 int join_post(b200conv* h) {
   CU_CHECK(h, cudaEventRecord(h->ev_join, h->s_post));
@@ -1799,6 +1816,7 @@ b200conv_t* b200conv_create(const b200conv_config* cfg) {
 
 void b200conv_destroy(b200conv_t* h) {
   if (!h) return;
+  swap_cancel(h);
   if (!h->sticky_cuda_error || h->s_main) {
     cudaSetDevice(h->cfg.device);
     if (h->s_main) cudaStreamSynchronize(h->s_main);
@@ -1842,6 +1860,7 @@ int b200conv_init_twostage(b200conv_t* h, size_t head_block, size_t tail_block,
                            const float* const* ir, const size_t* ir_len) {
   REQUIRE_CUDA(h);
   if (head_block == 0 || tail_block == 0) {                       // TwoStageFFTConvolver.cpp:94-97
+    if (h->swap_peer) return fail(h, B200CONV_ESTATE, "an IR hot swap is pending on this handle");
     if (int rc = set_device(h)) return rc;
     cudaStreamSynchronize(h->s_main);
     free_all(h);
@@ -1876,6 +1895,7 @@ static int init_shaped(b200conv_t* h, int n_stages, const size_t* blocks, const 
                        const float* const* raw, size_t n, const b200conv_ir_shape_params* sp,
                        const b200conv_ir_recalc_params* rp = nullptr) {
   if (!raw || (!sp && !rp)) return fail(h, B200CONV_EINVAL, "null argument");
+  if (h->swap_peer) return fail(h, B200CONV_ESTATE, "an IR hot swap is pending on this handle");
   if (h->C < 2 || h->C > 8) return fail(h, B200CONV_ESTATE, "IR shaping works on 2..8 channel handles (LL, RR[, LR, RL])");
   float* dev[8] = {};
   size_t m = 0, trimmed[8] = {}, lens[8] = {};
@@ -2328,6 +2348,30 @@ float chain_coeff(float freq, float srate) {
   return (a0 * t * t * t) + (a1 * t * t) + (a2 * t) + a3;
 }
 
+// samples per channel of the reference's warmer ring, (int)ceil(srate) / 4 (src/PluginProcessor.cpp:610)
+size_t chain_warmer_len(double srate) { return (size_t)((long long)std::ceil(srate) / 4); }
+
+// threads of k_chain_send for n samples: two passes of n/T sequential samples (~200 cycles each) + a serial scan of T
+// 8x8 matrix-vector steps (~256 cycles each): T ~ sqrt(1.5 n), a power of two in [8, 1024]
+int chain_send_threads(size_t n) {
+  int T = 8;
+  while (T < 1024 && (size_t)T * T < n + n / 2) T *= 2;
+  return T;
+}
+
+int launch_chain_send(b200conv* h, const pc::ChainSendParams& sp, cudaStream_t st) {
+  const int T = chain_send_threads((size_t)sp.n);
+#if defined(PC_EMULATE)
+  (void)st;
+  pc::emu_chain_send(sp, T);
+#else
+  pc::k_chain_send<<<2, T, 0, st>>>(sp);
+  CU_CHECK(h, cudaGetLastError());
+#endif
+  h->launches++;
+  return 0;
+}
+
 // Filter::init (src/dsp/Filter.cpp:3-21) with the q the processor passes (src/PluginProcessor.cpp:845-848)
 pc::ChainFilter chain_filter(bool on, int slope, int mode, float srate, float freq) {
   pc::ChainFilter f{};
@@ -2352,6 +2396,7 @@ pc::ChainFilter chain_filter(bool on, int slope, int mode, float srate, float fr
 
 int b200conv_chain_configure(b200conv_t* h, const b200conv_chain_config* cfg) {
   REQUIRE_CUDA(h);
+  if (h->swap_peer) return fail(h, B200CONV_ESTATE, "an IR hot swap is pending on this handle");
   if (!cfg) { h->chain_on = false; h->route_in_only = false; return B200CONV_OK; }
   if (h->C != 2 && h->C != 4) return fail(h, B200CONV_ESTATE, "the send / wet chain needs a stereo (C = 2) or quad (C = 4) handle");
   if (h->route_on) return fail(h, B200CONV_ESTATE, "the send / wet chain cannot be combined with b200conv_set_routing");
@@ -2366,12 +2411,15 @@ int b200conv_chain_configure(b200conv_t* h, const b200conv_chain_config* cfg) {
   h->chain_lc = chain_filter(cfg->lowcut_hz > 20.0f, cfg->lowcut_slope, 2, sr, cfg->lowcut_hz);          // HP, PluginProcessor.cpp:1643
   h->chain_hc = chain_filter(cfg->highcut_hz < 20000.0f, cfg->highcut_slope, 0, sr, cfg->highcut_hz);   // LP, :1647
   const size_t L = h->Lmax;
-  const size_t ring = next_pow2((size_t)cfg->predelay + L + 1);
+  // the ring doubles as the warmer of an IR hot swap (W = 0.25 s, src/PluginProcessor.cpp:610): the replay reads up to
+  // W samples behind the end of the call's first piece
+  const size_t ring = next_pow2(std::max((size_t)cfg->predelay, chain_warmer_len(cfg->srate)) + L + 1);
   if (!h->c_io) {
     CU_CHECK(h, cudaMalloc(&h->c_io, 6 * L * sizeof(float)));
     CU_CHECK(h, cudaMalloc(&h->c_conv_in, 2 * L * sizeof(float)));
-    CU_CHECK(h, cudaMalloc(&h->c_filt, 2 * L * sizeof(float)));
-    CU_CHECK(h, cudaMalloc(&h->c_state, 2 * pc::kChainStates * sizeof(float)));
+    CU_CHECK(h, cudaMalloc(&h->c_filt, 3 * L * sizeof(float)));
+    CU_CHECK(h, cudaMemsetAsync(h->c_filt + 2 * L, 0, L * sizeof(float), h->s_main));
+    CU_CHECK(h, cudaMalloc(&h->c_state, 4 * pc::kChainStates * sizeof(float)));
     CU_CHECK(h, cudaMallocHost((void**)&h->c_hpin, 6 * h->hpin_cap * sizeof(float)));
 #if defined(PC_EMULATE)
     h->c_hpin_dev = h->c_hpin;
@@ -2390,9 +2438,63 @@ int b200conv_chain_configure(b200conv_t* h, const b200conv_chain_config* cfg) {
   h->c_ring_pos = 0;
   for (int c = 0; c < 8; ++c) h->in_map[c] = c & 1;        // LL, RR, LR, RL <- L, R, L, R (StereoConvolver.cpp:35-40)
   h->chain_on = true;
+  h->swap_state = 0;
   CU_CHECK(h, cudaStreamSynchronize(h->s_main));
   return B200CONV_OK;
 }
+
+namespace {
+// one piece of a chain call through handle x's convolvers: LL, RR[, LR, RL] read rows in_map[c] of `in` (stride
+// in_stride); the per-convolver outputs stay in x->dch[0]
+int chain_convolve(b200conv* x, const float* in, size_t in_stride, size_t n) {
+  x->route_in_only = true;
+  int rc = 0;
+  if (const int nc = rt_cluster_ctas(x, n)) rc = rt_call(x, nc, in, in_stride, x->dch[0], x->Lmax, n, false);
+  else rc = run_group(x, in, in_stride, x->dch[0], x->Lmax, n, false);
+  x->route_in_only = false;
+  return rc;
+}
+
+// The warm-up of an IR hot swap (src/PluginProcessor.cpp:1694-1751), queued on g->s_main behind the send kernel of
+// the call's first piece: the replay of numBlocks * host_block samples from the ring, through fresh low / high cut
+// filters, into g's staging (LL, RR; zeros for LR / RL), then fed through g in batched launch groups.
+int chain_warm_up(b200conv* h, b200conv* g) {
+  const long long W = (long long)chain_warmer_len(h->chain_cfg.srate);
+  const long long N = W / (long long)h->swap_block * (long long)h->swap_block;
+  const size_t L = g->Lmax, chunk = L - g->stages[0].B;
+  if (N == 0) return 0;
+  float* rstate = h->c_state + 2 * pc::kChainStates;
+  CU_CHECK(g, cudaMemsetAsync(rstate, 0, 2 * pc::kChainStates * sizeof(float), g->s_main));
+  if (g->C > 2) CU_CHECK(g, cudaMemsetAsync(g->din[0] + 2 * L, 0, (size_t)(g->C - 2) * L * sizeof(float), g->s_main));
+  for (long long off = 0; off < N;) {
+    const long long n = std::min(N - off, (long long)chunk);
+    pc::ChainSendParams sp{};
+    sp.filt = g->din[0]; sp.filt_stride = (long long)L;
+    sp.state = rstate;
+    sp.ring = h->c_ring; sp.ring_stride = (long long)h->c_ring_size; sp.ring_mask = (long long)h->c_ring_size - 1;
+    sp.ring_pos = h->c_ring_pos; sp.n = n;
+    sp.lc = h->chain_lc; sp.hc = h->chain_hc;
+    sp.replay_w = W; sp.replay_off = off;
+    if (int rc = launch_chain_send(g, sp, g->s_main)) return rc;
+    if (int rc = run_group(g, g->din[0], L, g->dout[0], L, (size_t)n, false)) return rc;
+    off += n;
+  }
+  return 0;
+}
+
+// end of the fade: the chain (filter states, predelay / warmer ring, configuration, staging) moves to g by pointer
+void chain_move(b200conv* h, b200conv* g) {
+  std::swap(h->c_io, g->c_io); std::swap(h->c_conv_in, g->c_conv_in); std::swap(h->c_filt, g->c_filt);
+  std::swap(h->c_state, g->c_state); std::swap(h->c_hpin, g->c_hpin); std::swap(h->c_hpin_dev, g->c_hpin_dev);
+  std::swap(h->c_ring, g->c_ring); std::swap(h->c_ring_size, g->c_ring_size); std::swap(h->c_ring_pos, g->c_ring_pos);
+  g->chain_cfg = h->chain_cfg; g->chain_lc = h->chain_lc; g->chain_hc = h->chain_hc;
+  g->chain_on = true; h->chain_on = false;
+  for (int c = 0; c < 8; ++c) g->in_map[c] = c & 1;
+  h->swap_peer = g->swap_peer = nullptr;
+  h->swap_live = false;
+  h->swap_state = 3; g->swap_state = 0;
+}
+}  // namespace
 
 int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* ysend, const float* yrev, float* const* out, size_t len) {
   REQUIRE_CUDA(h);
@@ -2403,7 +2505,10 @@ int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* 
   if (int rc = set_device(h)) return rc;
   const int C = h->C;
   const size_t L = h->Lmax, B0 = h->stages[0].B;
-  const size_t chunk = L - B0;
+  b200conv* g = h->swap_live ? h->swap_peer : nullptr;        // incoming handle of a pending IR hot swap
+  const size_t chunk = g ? std::min(L - B0, L - (size_t)g->stages[0].B) : L - B0;
+  // the call in which the fade completes drops the LR / RL terms (deviation: DESIGN §5)
+  const bool completing = g && h->swap_xfade - (long long)len <= 0;
   float* d_dry = h->c_io; float* d_send = h->c_io + 2 * L; float* d_rev = h->c_io + 3 * L; float* d_out = h->c_io + 4 * L;
   // real-time calls: the kernels read the dry block + envelopes straight from pinned host memory and write the mix
   // back into it (zero-copy), so a callback is three launches and one synchronise instead of six copies more
@@ -2434,25 +2539,22 @@ int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* 
     sp.ring = h->c_ring; sp.ring_stride = (long long)h->c_ring_size; sp.ring_mask = (long long)h->c_ring_size - 1;
     sp.ring_pos = h->c_ring_pos; sp.predelay = h->chain_cfg.predelay; sp.n = (long long)n;
     sp.lc = h->chain_lc; sp.hc = h->chain_hc;
-    // chunks: two passes of n/T sequential samples (~200 cycles each) + a serial scan of T 8x8 matrix-vector steps
-    // (~256 cycles each): T ~ sqrt(1.5 n), a power of two in [8, 1024]
-    int T = 8;
-    while (T < 1024 && (size_t)T * T < n + n / 2) T *= 2;
-#if defined(PC_EMULATE)
-    pc::emu_chain_send(sp, T);
-#else
-    pc::k_chain_send<<<2, T, 0, h->s_main>>>(sp);
-    CU_CHECK(h, cudaGetLastError());
-#endif
-    h->launches++;
+    if (int rc = launch_chain_send(h, sp, h->s_main)) return rc;
     h->c_ring_pos = (h->c_ring_pos + (long long)n) & ((long long)h->c_ring_size - 1);
+    if (g) {
+      // the incoming handle runs on its own stream behind the send kernel: warm-up (first call), then this piece's
+      // undelayed send (src/PluginProcessor.cpp:1801-1806)
+      CU_CHECK(h, cudaEventRecord(h->ev_h2d[0], h->s_main));
+      CU_CHECK(g, cudaStreamWaitEvent(g->s_main, h->ev_h2d[0], 0));
+      if (h->swap_state == 1) {
+        if (int rc = chain_warm_up(h, g)) return rc;
+        h->swap_state = g->swap_state = 2;
+      }
+      if (int rc = chain_convolve(g, h->c_filt, L, n)) return rc;
+      CU_CHECK(g, cudaEventRecord(g->ev_comp[0], g->s_main));
+    }
     // the convolvers: LL, RR[, LR, RL] read the chain's L / R, per-convolver outputs stay on the device
-    h->route_in_only = true;
-    int rc = 0;
-    if (const int nc = rt_cluster_ctas(h, n)) rc = rt_call(h, nc, h->c_conv_in, L, h->dch[0], L, n, false);
-    else rc = run_group(h, h->c_conv_in, L, h->dch[0], L, n, false);
-    h->route_in_only = false;
-    if (rc) return rc;
+    if (int rc = chain_convolve(h, h->c_conv_in, L, n)) return rc;
     pc::ChainWetParams wp{};
     wp.dry = d_dry; wp.dry_stride = (long long)dstride;
     wp.conv = h->dch[0]; wp.conv_stride = (long long)L;
@@ -2460,10 +2562,19 @@ int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* 
     wp.out = d_out; wp.out_stride = (long long)dstride; wp.n = (long long)n;
     wp.quad_ts = (C == 4 && h->chain_cfg.true_stereo) ? 1 : 0;
     wp.width = h->chain_cfg.width; wp.drygain = h->chain_cfg.drygain; wp.wetgain = h->chain_cfg.wetgain;
+    if (g) {
+      CU_CHECK(h, cudaStreamWaitEvent(h->s_main, g->ev_comp[0], 0));
+      wp.conv_in = g->dch[0];
+      wp.xfade0 = h->swap_xfade; wp.xfadelen = h->swap_xfadelen;
+      if (completing) wp.quad_ts = 0;
+      h->swap_xfade -= (long long)n;
+    }
 #if defined(PC_EMULATE)
-    pc::emu_chain_wet(wp);
+    if (g) pc::emu_chain_wet_xfade(wp);
+    else pc::emu_chain_wet(wp);
 #else
-    pc::k_chain_wet<<<(unsigned)((n + 255) / 256), 256, 0, h->s_main>>>(wp);
+    if (g) pc::k_chain_wet_xfade<<<(unsigned)((n + 255) / 256), 256, 0, h->s_main>>>(wp);
+    else pc::k_chain_wet<<<(unsigned)((n + 255) / 256), 256, 0, h->s_main>>>(wp);
     CU_CHECK(h, cudaGetLastError());
 #endif
     h->launches++;
@@ -2475,8 +2586,40 @@ int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* 
       for (int ch = 0; ch < 2; ++ch) std::memcpy(out[ch], h->c_hpin + (4 + ch) * h->hpin_cap, n * sizeof(float));
     done += n;
   }
+  if (g && h->swap_xfade <= 0) chain_move(h, g);        // src/PluginProcessor.cpp:1823-1826
   return B200CONV_OK;
 }
+
+int b200conv_chain_swap(b200conv_t* live, b200conv_t* incoming, size_t host_block) {
+  REQUIRE_CUDA(live);
+  REQUIRE_CUDA(incoming);
+  if (live == incoming) return fail(live, B200CONV_EINVAL, "the IR hot swap needs two different handles");
+  if (live->cfg.device != incoming->cfg.device) return fail(live, B200CONV_EINVAL, "the IR hot swap needs both handles on one device");
+  if (live->cfg.shard_count > 1 || incoming->cfg.shard_count > 1 || live->route_on || incoming->route_on ||
+      live->p2p_on || incoming->p2p_on)
+    return fail(live, B200CONV_EINVAL, "the IR hot swap needs unsharded handles without I/O routing");
+  if (host_block == 0) return fail(live, B200CONV_EINVAL, "host_block 0");
+  if (!live->chain_on) return fail(live, B200CONV_ESTATE, "the live handle has no send / wet chain");
+  if (incoming->stages.empty()) return fail(live, B200CONV_ESTATE, "the incoming handle has no impulse response");
+  if (incoming->chain_on) return fail(live, B200CONV_ESTATE, "the incoming handle already owns a send / wet chain");
+  if (live->swap_peer || incoming->swap_peer) return fail(live, B200CONV_ESTATE, "an IR hot swap is already pending");
+  if (incoming->C != 2 && incoming->C != 4)
+    return fail(live, B200CONV_ESTATE, "the send / wet chain needs a stereo (C = 2) or quad (C = 4) handle");
+  if (live->Lmax != incoming->Lmax || live->hpin_cap != incoming->hpin_cap)
+    return fail(live, B200CONV_EINVAL, "the IR hot swap needs equal staging sizes (same head block and batch size)");
+  live->swap_peer = incoming; incoming->swap_peer = live;
+  live->swap_live = true; incoming->swap_live = false;
+  live->swap_state = incoming->swap_state = 1;
+  live->swap_block = host_block;
+  // src/PluginProcessor.cpp:1754-1755
+  live->swap_xfadelen = (long long)std::ceil(live->chain_cfg.srate * 50 / 1000.0);
+  live->swap_xfade = live->swap_xfadelen;
+  // during the warm-up and the fade only LL and RR get input; LR / RL of a quad handle read c_filt's zero row
+  for (int c = 0; c < 8; ++c) incoming->in_map[c] = c < 2 ? c : 2;
+  return B200CONV_OK;
+}
+
+int b200conv_chain_swap_state(const b200conv_t* h) { return h ? h->swap_state : 0; }
 
 int b200conv_clear(b200conv_t* h) {
   REQUIRE_CUDA(h);
@@ -2497,7 +2640,9 @@ int b200conv_reset(b200conv_t* h) {
   CU_CHECK(h, cudaStreamSynchronize(h->s_main));
   CU_CHECK(h, cudaStreamSynchronize(h->s_post));
   if (h->s_tail) CU_CHECK(h, cudaStreamSynchronize(h->s_tail));
+  swap_cancel(h);
   free_all(h);
+  h->swap_state = 0;
   return B200CONV_OK;
 }
 
