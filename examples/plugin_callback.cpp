@@ -2,7 +2,9 @@
 // loader thread: raw IR -> b200conv_init_twostage_shaped (shaping + partition spectra on the GPU, one upload);
 // audio thread:  one b200conv_chain_process per callback (dry L/R + the two envelopes in, final mix out) instead of
 //                src/PluginProcessor.cpp:1639-1653 (send + filters), :1766-1790 (predelay), :1793 (4 convolvers),
-//                :1832-1876 (mixdown, reverb envelope, width, dry/wet).
+//                :1832-1876 (mixdown, reverb envelope, width, dry/wet); knob moves (an automated dry/wet ramp and
+//                low-cut sweep here) go in with b200conv_chain_update before the callback's process call, as
+//                onSlider / the per-block parameter reads do (:1151-1233), without resetting filters or predelay.
 // The second half cross-checks the wet path against four drop-in convolver objects mixed on the host the reference's way.
 //
 //   g++ -O2 -std=c++17 -I include examples/plugin_callback.cpp -L reevr_b200 -l:libb200conv.so \
@@ -61,6 +63,12 @@ int main()
   std::vector<float> outL(n), outR(n);
   for (size_t pos = 0; pos < n; pos += hostBlock)
   {
+    // automation: dry/wet from 0.2 to 0.8 (equal-power gains, :1177-1182) and the low cut from 80 Hz to 600 Hz
+    const float u = static_cast<float>(pos) / static_cast<float>(n - hostBlock);
+    const float theta = (0.2f + 0.6f * u) * 1.57079632679f;
+    b200conv_chain_config knob = cc;
+    knob.drygain = std::cos(theta); knob.wetgain = std::sin(theta); knob.lowcut_hz = 80.0f + 520.0f * u;
+    if (b200conv_chain_update(h, &knob) != B200CONV_OK) { std::printf("update: %s\n", b200conv_last_error(h)); return 2; }
     const float* dry[2] = { &L[pos], &R[pos] };
     float* out[2] = { &outL[pos], &outR[pos] };
     if (b200conv_chain_process(h, dry, &ysend[pos], &yrev[pos], out, hostBlock) != B200CONV_OK)

@@ -159,7 +159,8 @@ int b200conv_set_routing(b200conv_t* h, int n_in, const int* in_map, int n_out, 
  *         (src/PluginProcessor.cpp:1832-1876).
  * dry[2] / out[2]: host L, R; ysend / yrev: per-sample send and reverb envelopes (NULL = 1).  One H2D of the dry
  * signal + envelopes and one D2H of the final mix per call, whatever the number of convolvers.
- * b200conv_chain_configure(h, cfg) after the IR is loaded (resets filter states and the delay line; NULL disables). */
+ * b200conv_chain_configure(h, cfg) after the IR is loaded (resets filter states and the delay line; NULL disables);
+ * b200conv_chain_update(h, cfg) for parameter changes while playing. */
 typedef struct b200conv_chain_config {
   double srate;
   float lowcut_hz;  int lowcut_slope;
@@ -169,6 +170,25 @@ typedef struct b200conv_chain_config {
   int true_stereo;              /* quad handles: add RL to the left and LR to the right */
 } b200conv_chain_config;
 int b200conv_chain_configure(b200conv_t* h, const b200conv_chain_config* cfg);
+/* New chain parameters without a reset: what REEV-R's onSlider and the per-block parameter reads of processBlock do
+ * (src/PluginProcessor.cpp:837-848, 1151-1188).  b200conv_chain_configure is prepareToPlay: it clears the filters and
+ * the delay line.  b200conv_chain_update takes the same struct and applies it from the start of the next
+ * b200conv_chain_process call (once per call, however the call is cut into pieces):
+ *   - cut frequencies / slopes: new coefficients, filter state continues; a filter switched off keeps its state; each
+ *     filter keeps the reference's separate 6 dB and 12 / 24 dB state variables across slope switches;
+ *   - predelay: the delay history is kept and read at the new delay.  The delay line has the reference's length
+ *     D = (int)(2 * srate); a predelay beyond D sets D = 2 * predelay and the delay history reads zero from there
+ *     (the reference clears its delay line), while the send history an IR hot swap replays is kept;
+ *   - width, drygain, wetgain, true_stereo: from the next call, including the crossfade of a pending swap.
+ * It applies to the handle that owns the chain, including the live handle while a swap is pending (an update before
+ * the warm-up call changes the filters the warm-up replays through); at the end of the fade the configuration moves to
+ * the incoming handle with the chain.
+ * Real-time safe: no CUDA call, allocation, synchronise or launch.  The one exception is a predelay that grows the
+ * delay line past what the device ring holds: the ring is then reallocated (synchronising the handle's streams).
+ * B200CONV_ESTATE: the handle owns no chain (never configured, the incoming handle of a pending swap, or a handle that
+ * gave its chain away).  B200CONV_EINVAL: cfg == NULL, a slope outside 0..2, predelay < 0, or an srate different from
+ * the configured one (a new rate needs b200conv_chain_configure).  On any error nothing changes. */
+int b200conv_chain_update(b200conv_t* h, const b200conv_chain_config* cfg);
 int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* ysend, const float* yrev,
                            float* const* out, size_t len);
 

@@ -187,6 +187,16 @@ class Engine:
                                int(true_stereo))
         self._check(self._l.b200conv_chain_configure(self._h, C.byref(cfg)), "chain_configure")
 
+    def chain_update(self, srate: float, lowcut_hz: float = 20.0, lowcut_slope: int = 0, highcut_hz: float = 20000.0,
+                     highcut_slope: int = 0, predelay: int = 0, width: float = 1.0, drygain: float = 1.0,
+                     wetgain: float = 1.0, true_stereo: bool = True) -> None:
+        """New chain parameters from the next chain_process call on, keeping the filter states and the delay history
+        (b200conv_chain_update; what the reference's onSlider and per-block parameter reads do).  srate must be the
+        configured rate."""
+        cfg = _lib.ChainConfig(srate, lowcut_hz, lowcut_slope, highcut_hz, highcut_slope, predelay, width, drygain, wetgain,
+                               int(true_stereo))
+        self._check(self._l.b200conv_chain_update(self._h, C.byref(cfg)), "chain_update")
+
     def chain_process(self, dryL, dryR, ysend=None, yrev=None):
         """(outL, outR) = drygain * dry + wetgain * width(yrev * mixdown(convolvers(predelay(filters(dry * ysend)))))"""
         xs = [np.ascontiguousarray(a, dtype=np.float32) for a in (dryL, dryR)]
