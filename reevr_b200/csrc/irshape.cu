@@ -350,36 +350,44 @@ struct SvfCoeffs {
   float g, r2, a1, a2, a3, cl, cb, ch;
 };
 constexpr int kSvfHP6 = 7, kSvfLP6 = 8;
-PC_HD float svf_step(const SvfCoeffs& f, float* s, float x) {
+// F = float: the reference's arithmetic.  F = double: the same equations from the same float coefficients (A^L)
+template <class F>
+PC_HD F svf_step(const SvfCoeffs& f, F* s, F x) {
   if (f.mode == kSvfHP6 || f.mode == kSvfLP6) {
-    const float delta = f.g * (x - s[0]);
+    const F delta = (F)f.g * (x - s[0]);
     s[0] += delta;
     return f.mode == kSvfLP6 ? s[0] : x - s[0];
   }
-  const float v3 = x - s[1];
-  const float v1 = f.a1 * s[0] + f.a2 * v3;
-  const float v2 = s[1] + f.a2 * s[0] + f.a3 * v3;
-  s[0] = 2.0f * v1 - s[0];
-  s[1] = 2.0f * v2 - s[1];
-  return f.cl * v2 + f.cb * v1 + f.ch * (x - f.r2 * v1 - v2);
+  const F v3 = x - s[1];
+  const F v1 = (F)f.a1 * s[0] + (F)f.a2 * v3;
+  const F v2 = s[1] + (F)f.a2 * s[0] + (F)f.a3 * v3;
+  s[0] = (F)2 * v1 - s[0];
+  s[1] = (F)2 * v2 - s[1];
+  return (F)f.cl * v2 + (F)f.cb * v1 + (F)f.ch * (x - (F)f.r2 * v1 - v2);
 }
 // one section in place over C channels (channel stride `stride`), state s = (s1, s2) from zero (SVF::clear(0), :247-251)
 struct SvfRec {
   using T = float;
   float* x; long long stride;
   SvfCoeffs f;
-  PC_HD float step(int ch, long long i, float* s) const { return svf_step(f, s, x[ch * stride + i]); }
-  PC_HD void free_step(float* s) const { (void)svf_step(f, s, 0.0f); }
+  PC_HD float step(int ch, long long i, float* s) const { return svf_step<float>(f, s, x[ch * stride + i]); }
+  PC_HD void free_step(double* s) const { (void)svf_step<double>(f, s, 0.0); }
   PC_HD void put(int ch, long long i, float v) const { x[ch * stride + i] = v; }
 };
 
-// ---- chunked form of a 2-state linear recursion, the scheme of k_chain_send (kernels_chain.cuh:9-20) ----
+// ---- chunked form of a 2-state linear recursion, the scheme of k_chain_send (kernels_chain.cuh:14-33) ----
 // kScanThreads chunks of L = ceil(n / kScanThreads) samples per channel: pass 1 runs every chunk from a zero state,
 // A^L comes from the zero-input response to the unit states, one thread scans S_{t+1} = A^L S_t + Z_t from S_0 = 0
-// (every channel starts from a zero state), pass 2 re-runs every chunk from its true state and writes.  The
-// resampler's flush of |y| <= 1e-8 to zero is the one non-linear step; it is applied inside the chunks (both passes), so
-// this is the one place where the chunked form can differ from the serial one: by less than 1e-8 per sample, fed into
-// a stable filter.  The split into chunks otherwise only re-associates the recurrence.
+// (every channel starts from a zero state), pass 2 re-runs every chunk from its true state and writes.
+// Precision: the chunks run in the recursion's own type (float for the SVF, in the reference's order; double for the
+// resampler); A^L (the zero-input response of the same step equations) and the scan always run in double, and the
+// states handed to pass 2 are rounded to the chunk type.  A low band at 96 / 192 kHz puts the poles within ~1e-4 of
+// the unit circle, where an error in S_t persists for tens of chunks: with A^L and the scan in float the SVF chunked
+// form was up to 5e-5 of peak from a float64 serial filter, 20-30x the serial float filter's own error; with them in
+// double it was 3e-7 for a 20 Hz, Q 8, +24 dB low shelf at 96 kHz (serial float: 1.6e-6) and never more than 1.7x
+// the serial float filter's error (tests/test_scan_precision.py).  The resampler's flush of |y| <= 1e-8 to zero is
+// the one non-linear step; it is applied inside the chunks (both passes), so the chunked form can differ from the
+// serial one there by less than 1e-8 per sample, fed into a stable filter.
 constexpr int kScanThreads = 1024;
 
 PC_HD void scan_bounds(int t, long long L, long long n, long long& i0, long long& i1) {
@@ -394,20 +402,21 @@ PC_HD void scan_chunk(const R& rec, int ch, long long i0, long long i1, typename
   }
 }
 template <class R>
-PC_HD void scan_power_column(const R& rec, long long L, int j, typename R::T* col) {
+PC_HD void scan_power_column(const R& rec, long long L, int j, double* col) {
   col[0] = j == 0 ? 1 : 0;
   col[1] = j == 1 ? 1 : 0;
   for (long long i = 0; i < L; ++i) rec.free_step(col);
 }
-// Z[t]: zero-state end point of chunk t on entry, the initial state of chunk t on exit; AL[q][j] = (A^L)_qj
+// Z[t]: zero-state end point of chunk t on entry, the initial state of chunk t (rounded to T) on exit;
+// AL[q][j] = (A^L)_qj; the scan runs in double
 template <class T>
-PC_HD void scan_states(T (*Z)[2], T (*AL)[2], int nt, long long L, long long n) {
-  T s0 = 0, s1 = 0;
+PC_HD void scan_states(T (*Z)[2], const double (*AL)[2], int nt, long long L, long long n) {
+  double s0 = 0, s1 = 0;
   for (int c = 0; c < nt; ++c) {
-    const T n0 = Z[c][0] + AL[0][0] * s0 + AL[0][1] * s1;
-    const T n1 = Z[c][1] + AL[1][0] * s0 + AL[1][1] * s1;
-    Z[c][0] = s0;
-    Z[c][1] = s1;
+    const double n0 = (double)Z[c][0] + AL[0][0] * s0 + AL[0][1] * s1;
+    const double n1 = (double)Z[c][1] + AL[1][0] * s0 + AL[1][1] * s1;
+    Z[c][0] = (T)s0;
+    Z[c][1] = (T)s1;
     if ((long long)c * L + L <= n) { s0 = n0; s1 = n1; }      // a ragged / empty last chunk does not advance by A^L
   }
 }
@@ -417,7 +426,7 @@ PC_HD void scan_states(T (*Z)[2], T (*AL)[2], int nt, long long L, long long n) 
 template <class R>
 __global__ void __launch_bounds__(kScanThreads) k_scan2(R rec, long long n) {
   using T = typename R::T;
-  __shared__ T AL[2][2];
+  __shared__ double AL[2][2];
   __shared__ T Z[kScanThreads][2];
   const int ch = blockIdx.x, t = threadIdx.x;
   const long long L = (n + kScanThreads - 1) / kScanThreads;
@@ -428,7 +437,7 @@ __global__ void __launch_bounds__(kScanThreads) k_scan2(R rec, long long n) {
   Z[t][0] = s[0];
   Z[t][1] = s[1];
   if (t < 2) {
-    T col[2];
+    double col[2];
     scan_power_column(rec, L, t, col);
     AL[0][t] = col[0];
     AL[1][t] = col[1];
@@ -481,7 +490,7 @@ void emu_scan2(const R& rec, int C, long long n) {
   const long long L = (n + kScanThreads - 1) / kScanThreads;
   std::vector<T> zbuf(2 * kScanThreads);
   T (*Z)[2] = reinterpret_cast<T (*)[2]>(zbuf.data());
-  T AL[2][2];
+  double AL[2][2];
   for (int ch = 0; ch < C; ++ch) {
     long long i0, i1;
     for (int t = 0; t < kScanThreads; ++t) {
@@ -492,7 +501,7 @@ void emu_scan2(const R& rec, int C, long long n) {
       Z[t][1] = s[1];
     }
     for (int j = 0; j < 2; ++j) {
-      T col[2];
+      double col[2];
       scan_power_column(rec, L, j, col);
       AL[0][j] = col[0];
       AL[1][j] = col[1];
