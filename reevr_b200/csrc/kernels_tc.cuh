@@ -12,11 +12,15 @@
 // and channel.  The complex product becomes real GEMMs by stacking [Hr ; Hi] into M = 128 rows and running the
 // same A against the real and the imaginary time line (two accumulators D, D2):
 //   y.re = D[0:64] - D2[64:128],  y.im = D[64:128] + D2[0:64]        (entry 0 = DC / Nyquist: y = (D[0:64], D2[64:128]))
-// Consumer warpgroup w of the sweep owns rows 64 w .. 64 w + 63 (w = 0: Hr, w = 1: Hi) of both accumulators.
+// The sweep issues the transposed product D^T[n][i] = sum_j B[j][n] * A[i][j]: the wgmma A operand is the time-line
+// window (M = 64 segments), the wgmma B operand the whole 128 x 32 Toeplitz image (N = 128), so every m64n128k8 reads
+// 2 KB + 4 KB of shared memory for 64 K FMA (an m64n64k8 reads 4 KB for 32 K FMA, which at the tf32 rate is the whole
+// shared-memory port).  Consumer warpgroup w owns time line w (re, im), i.e. accumulator D (w = 0) or D2 (w = 1), all
+// 128 rows.
 // FP32 accuracy comes from the 3xTF32 split: a = a_hi + a_lo, b = b_hi + b_lo (each tf32-exact), and
 // a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi accumulated in FP32 (dropped term ~2^-22 relative).
 //
-// The B operand of chunk c (32 values of j) is a ROW-SHIFTED WINDOW of one shared-memory strip.  The bin's time
+// The time-line operand of chunk c (32 values of j) is a ROW-SHIFTED WINDOW of one shared-memory strip.  The bin's time
 // line is stored as rows of 64 samples; plane e in {0, 1} holds the 32-sample half rows (128 B, SWIZZLE_128B
 // K-major).  B[32c + jj][n] = x[64 (n + c/2) + 32 (c%2) + jj - Q] is row n + c/2 of plane c%2, i.e. the same strip
 // with the descriptor start address advanced by (c/2) * 128 bytes: the 128-byte swizzle is a function of the
@@ -27,7 +31,7 @@
 // ring) stream during the tile.
 //
 // Kernels: k_tc_build_a (H -> tf32 hi/lo Toeplitz tile images, once per IR), k_tc_split_x (timeline rows -> per-bin
-// hi/lo time lines), k_tc_sweep (bulk-copy producer warp / two MMA warpgroups accumulating in registers),
+// hi/lo time lines), k_tc_sweep (bulk-copy producer warpgroup / two MMA warpgroups accumulating in registers),
 // k_tc_merge_y (partial planes -> Y rows, combines the complex product).
 #pragma once
 
@@ -45,7 +49,8 @@ constexpr int kStripBytes = kStripRows * 128;       // 10240 (a multiple of the 
 constexpr int kATileBytes = 128 * 128;              // one 128 x 32 tf32 Toeplitz tile image
 constexpr int kAStages = 4;
 constexpr int kSmemBytes = 8 * kStripBytes + kAStages * kATileBytes + 1024;
-constexpr int kThreads = 288;                       // two MMA warpgroups + one producer warp
+constexpr int kThreads = 384;                       // two MMA warpgroups + a producer warpgroup (one thread issues the copies)
+constexpr int kMmaRegs = 232, kProducerRegs = 40;   // setmaxnreg split of the register file: 256 x 232 + 128 x 40 <= 64 K
 constexpr int kFlush = 4;                           // K chunks accumulated by the tensor core before the FP32 register add
 
 struct Geom {
@@ -226,29 +231,32 @@ __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr & 0
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 // keeps the compiler from moving or copying accumulator registers across the wgmma issue / wait points
-__device__ __forceinline__ void fence_operands(float (&d)[2][32]) {
+__device__ __forceinline__ void fence_operands(float (&d)[64]) {
 #pragma unroll
-  for (int comp = 0; comp < 2; ++comp)
-#pragma unroll
-    for (int j = 0; j < 32; ++j) asm volatile("" : "+f"(d[comp][j]) :: "memory");
+  for (int j = 0; j < 64; ++j) asm volatile("" : "+f"(d[j]) :: "memory");
 }
 template <int N>
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
-// d[64 x 64] (+)= A[64 x 8] * B[8 x 64], tf32 operands from shared memory, FP32 accumulators in 32 registers per thread
-__device__ __forceinline__ void mma_tf32(float (&d)[32], uint32_t a_lo, uint32_t b_lo, uint32_t accumulate) {
+// d[64 x 128] (+)= A[64 x 8] * B[8 x 128], tf32 operands from shared memory, FP32 accumulators in 64 registers per thread
+__device__ __forceinline__ void mma_tf32(float (&d)[64], uint32_t a_lo, uint32_t b_lo, uint32_t accumulate) {
   const uint64_t da = ((uint64_t)kDescHi << 32) | a_lo, db = ((uint64_t)kDescHi << 32) | b_lo;
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
-               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
-               "%32, %33, p, 1, 1;\n\t}"
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+               "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+               "%64, %65, p, 1, 1;\n\t}"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
                  "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
                  "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
-                 "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+                 "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+                 "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+                 "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
                : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
 
-// grid: any (persistent, tiles walked round-robin); block 288 = MMA warpgroups 0 and 1 (warps 0-7), producer warp 8.
+// grid: any (persistent, tiles walked round-robin); block 384 = MMA warpgroups 0 and 1 (warps 0-7), producer
+// warpgroup 2 (warp 8 lane 0 issues the copies; the warpgroup exists so that setmaxnreg can hand its registers over).
 // Each MMA warpgroup accumulates the products of kFlush chunks in its wgmma registers and adds them to FP32
 // registers (round-to-nearest) between groups: the tensor core's accumulate truncates, so short accumulation chains
 // keep the error at the level of the FFMA sweep (tools/tc_accuracy_model.py).
@@ -268,8 +276,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_tc_sweep(SweepParams P) {
   __syncthreads();
   const int total = P.lines * P.ntile;
 
-  if (warp == 8) {
-    if (lane == 0) {                                      // ---- producer
+  if (warp >= 8) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(kProducerRegs));
+    if (warp == 8 && lane == 0) {                         // ---- producer
       unsigned it_a = 0;
       int n = 0;
       bool ok = true;
@@ -294,81 +303,100 @@ __global__ void __launch_bounds__(kThreads, 1) k_tc_sweep(SweepParams P) {
     return;
   }
 
-  // ---- MMA warpgroup `part` (rows 64 part .. 64 part + 63 of the stacked [Hr ; Hi] Toeplitz tile)
-  const int part = warp >> 2, wq = warp & 3;
+  // ---- MMA warpgroup `comp` (time line re / im against all 128 rows of the stacked [Hr ; Hi] Toeplitz tile)
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(kMmaRegs));   // two accumulator sets + the FP32 sums
+  const int comp = warp >> 2, wq = warp & 3;
   const bool leader = (tid & 127) == 0;
-  const uint32_t strip_lo = desc_lo(smem_addr(strips)), ring_lo = desc_lo(smem_addr(ring)) + (uint32_t)part * (8192u >> 4);
+  const uint32_t strip_lo = desc_lo(smem_addr(strips)), ring_lo = desc_lo(smem_addr(ring));
   unsigned it_a = 0;
   int n = 0;
-  float d[2][32];
+  // Accumulation chains alternate between d0 and d1: the chain of group g is folded into acc once the first stage of
+  // group g + 1 has been committed, so the tensor core keeps working on g + 1 while g drains and is added (same chains,
+  // same order of the FP32 adds as draining each chain before the next one starts).
+  float d0[64], d1[64];
 #pragma unroll
-  for (int comp = 0; comp < 2; ++comp)
+  for (int j = 0; j < 64; ++j) { d0[j] = 0.0f; d1[j] = 0.0f; }
+  float acc[64];
+  int pending = -1;                                       // ring stage whose MMAs may still be in flight
+  // issues chunks [g0, min(g0 + kFlush, nchunk)) into d; folds `prev` (the previous chain, if g0 > 0) into acc as soon
+  // as it is complete.  false: a barrier wait gave up
+  auto chain = [&](float (&d)[64], float (&prev)[64], int g0) -> bool {
+    const int gend = min(g0 + kFlush, P.nchunk);
+    for (int c = g0; c < gend; ++c) {
+      if (c < 2 && !mbar_wait(&bar_strip_full[c], (unsigned)n & 1u)) { if (leader) *reinterpret_cast<volatile int*>(P.err) = 3; return false; }
+      const uint32_t e = (uint32_t)c & 1u, q = (uint32_t)c >> 1;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) d[comp][j] = 0.0f;
-  for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++n) {
-    const int line = tile / P.ntile, nt = tile - line * P.ntile;
-    float acc[2][32];
+      for (int hl = 0; hl < 2; ++hl, ++it_a) {
+        const unsigned stage = it_a % kAStages, use = it_a / kAStages;
+        if (!mbar_wait(&bar_a_full[stage], use & 1u)) { if (leader) *reinterpret_cast<volatile int*>(P.err) = 5; return false; }
+        __syncwarp();                                     // wgmma is .aligned: the warp issues it converged
+        fence_operands(d);
+        wg_fence();
+        const uint32_t img = ring_lo + stage * (kATileBytes >> 4);
 #pragma unroll
-    for (int comp = 0; comp < 2; ++comp)
-#pragma unroll
-      for (int j = 0; j < 32; ++j) acc[comp][j] = 0.0f;
-    for (int g0 = 0; g0 < P.nchunk; g0 += kFlush) {      // one accumulation chain per group of kFlush chunks
-      const int gend = min(g0 + kFlush, P.nchunk);
-      int pending = -1;                                   // ring stage whose MMAs may still be in flight
-      for (int c = g0; c < gend; ++c) {
-        if (c < 2 && !mbar_wait(&bar_strip_full[c], (unsigned)n & 1u)) { if (leader) *reinterpret_cast<volatile int*>(P.err) = 3; wg_wait<0>(); return; }
-        const uint32_t e = (uint32_t)c & 1u, q = (uint32_t)c >> 1;
-#pragma unroll
-        for (int hl = 0; hl < 2; ++hl, ++it_a) {
-          const unsigned stage = it_a % kAStages, use = it_a / kAStages;
-          if (!mbar_wait(&bar_a_full[stage], use & 1u)) { if (leader) *reinterpret_cast<volatile int*>(P.err) = 5; wg_wait<0>(); return; }
-          __syncwarp();                                   // wgmma is .aligned: the warp issues it converged
-          fence_operands(d);
-          wg_fence();
-          const uint32_t a_lo = ring_lo + stage * (kATileBytes >> 4);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-            for (int comp = 0; comp < 2; ++comp) {
-              const uint32_t bhi = strip_lo + (((comp * 2 + 0) * 2 + e) * kStripBytes >> 4) + q * 8 + kk * 2;
-              const uint32_t blo = strip_lo + (((comp * 2 + 1) * 2 + e) * kStripBytes >> 4) + q * 8 + kk * 2;
-              if (hl == 0) {
-                mma_tf32(d[comp], a_lo + kk * 2, bhi, (c > g0 || kk > 0) ? 1u : 0u);
-                mma_tf32(d[comp], a_lo + kk * 2, blo, 1u);
-              } else {
-                mma_tf32(d[comp], a_lo + kk * 2, bhi, 1u);
-              }
-            }
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint32_t xhi = strip_lo + (((comp * 2 + 0) * 2 + e) * kStripBytes >> 4) + q * 8 + kk * 2;
+          const uint32_t xlo = strip_lo + (((comp * 2 + 1) * 2 + e) * kStripBytes >> 4) + q * 8 + kk * 2;
+          if (hl == 0) {
+            mma_tf32(d, xhi, img + kk * 2, (c > g0 || kk > 0) ? 1u : 0u);
+            mma_tf32(d, xlo, img + kk * 2, 1u);
+          } else {
+            mma_tf32(d, xhi, img + kk * 2, 1u);
           }
-          wg_commit();
-          fence_operands(d);
-          wg_wait<1>();                                   // the previous stage's MMAs are done: hand it back
-          fence_operands(d);
-          if (leader && pending >= 0) mbar_arrive1(&bar_a_empty[pending]);
-          pending = (int)stage;
+        }
+        wg_commit();
+        fence_operands(d);
+        wg_wait<1>();                                     // everything before this stage's MMAs is done
+        fence_operands(d);
+        if (leader && pending >= 0) mbar_arrive1(&bar_a_empty[pending]);
+        pending = (int)stage;
+        if (c == g0 && hl == 0 && g0 > 0) {               // the previous chain is complete: fold it
+          fence_operands(prev);
+#pragma unroll
+          for (int j = 0; j < 64; ++j) acc[j] += prev[j];
         }
       }
-      wg_wait<0>();                                       // the chain is complete: fold it into FP32 registers
-      fence_operands(d);
-      if (leader) {
-        mbar_arrive1(&bar_a_empty[pending]);
-        if (gend == P.nchunk) mbar_arrive1(&bar_strip_empty);
-      }
-#pragma unroll
-      for (int comp = 0; comp < 2; ++comp)
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[comp][j] += d[comp][j];
     }
-    // accumulator fragment of m64n64: register 4 j + r of lane l in warp wq holds row 16 wq + l / 4 + 8 (r / 2),
-    // column 8 j + 2 (l % 4) + (r % 2)
-    const int i0 = 16 * wq + (lane >> 2), n0 = 2 * (lane & 3);
+    return true;
+  };
+  for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++n) {
+    const int line = tile / P.ntile, nt = tile - line * P.ntile;
 #pragma unroll
-    for (int comp = 0; comp < 2; ++comp) {
+    for (int j = 0; j < 64; ++j) acc[j] = 0.0f;
+    for (int g0 = 0; g0 < P.nchunk; g0 += 2 * kFlush) {  // one accumulation chain per group of kFlush chunks
+      if (!chain(d0, d1, g0)) { wg_wait<0>(); return; }
+      if (g0 + kFlush >= P.nchunk) break;
+      if (!chain(d1, d0, g0 + kFlush)) { wg_wait<0>(); return; }
+    }
+    wg_wait<0>();                                         // the last chain is complete: fold it, hand back the strips
+    fence_operands(d0);
+    fence_operands(d1);
+    if (leader) {
+      mbar_arrive1(&bar_a_empty[pending]);
+      mbar_arrive1(&bar_strip_empty);
+    }
+    pending = -1;
+    if ((P.nchunk + kFlush - 1) / kFlush & 1) {           // an odd number of chains ends in d0
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc[j] += d0[j];
+    } else {
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc[j] += d1[j];
+    }
+    // accumulator fragment of m64n128: register 4 j + r of lane l in warp wq holds segment 16 wq + l / 4 + 8 (r / 2) and
+    // Toeplitz row m = 8 j + 2 (l % 4) + (r % 2), i.e. output step m % 64 of plane comp * 2 + m / 64; registers 4 j + r
+    // and 4 j + r + 1 (r even) are consecutive steps
+    const int n0 = 16 * wq + (lane >> 2), i0 = 2 * (lane & 3);
+#pragma unroll
+    for (int part = 0; part < 2; ++part) {
       float* dst = P.Yt + ((size_t)line * 4 + comp * 2 + part) * P.Lty + (size_t)nt * kN * 64;
 #pragma unroll
       for (int j = 0; j < 8; ++j)
 #pragma unroll
-        for (int r = 0; r < 4; ++r) dst[(size_t)(8 * j + n0 + (r & 1)) * 64 + i0 + 8 * (r >> 1)] = acc[comp][4 * j + r];
+        for (int h = 0; h < 2; ++h) {
+          const int r = 4 * (8 * part + j) + 2 * h;
+          *reinterpret_cast<float2*>(dst + (size_t)(n0 + 8 * h) * 64 + 8 * j + i0) = make_float2(acc[r], acc[r + 1]);
+        }
     }
   }
 }
