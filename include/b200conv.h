@@ -123,7 +123,13 @@ int b200conv_last_sweep_variant(const b200conv_t* h);
  * but 0 of a steady batch job — until the next b200conv_clear), "stream_alternate" (default 1: the streaming sweep
  * walks its partition slices in alternating directions from launch to launch, see kernels_stream.cuh), "tc" (default 1:
  * launch groups of >= 4096 blocks with <= 961 partitions run the sweep on the tensor cores, kernels_tc.cuh; 0 = always
- * the packed-FMA sweep). */
+ * the packed-FMA sweep).
+ * "shard_head" (sharded handles; set before b200conv_init_*, B200CONV_ESTATE once an IR is loaded; default 1 = every
+ * stage partition-range sharded): 0 = tail layout — shard 0 holds the head stage (stage 0) whole and keeps the one-launch
+ * real-time call, the other shards hold none of it (no head FFT, sweep or output, only the input buffering of the
+ * later stages), and only the stages >= 1 are partition-range sharded.  Their partial spectra are summed on shard 0 by
+ * the reduce hook, called once per completed tail block (one row of C*B complex bins) and never for the head, or by the
+ * tail slot exchange (b200conv_p2p_export / import below).  Applies to every init, up to 4 stages. */
 int    b200conv_set_option(b200conv_t* h, const char* name, int value);
 /* Device time (ms) spent in the dominant CMAC kernel / all kernels during the last
  * b200conv_process_device call, measured with CUDA events on the handle's stream
@@ -228,7 +234,13 @@ int b200conv_process_xfade(b200conv_t* h_old, b200conv_t* h_new, const float* co
  * and writes the audio directly into shard 0's output exchange buffer.  No NCCL call on the data
  * path.  Set-up: every shard exports a blob, the caller all-gathers the blobs (rank order) and
  * every shard imports the concatenation.  mode 0 = CUDA IPC handles (one process per GPU),
- * mode 1 = raw pointers (all shards in one process on one device; tests). */
+ * mode 1 = raw pointers (all shards in one process on one device; tests).
+ * Handles with shard_head = 0 (any stage schedule) attach the TAIL slot exchange instead: the single-block sweep of
+ * every tail block stores this shard's partial spectrum into its slot on shard 0 and raises its flag; shard 0 waits for
+ * the flags on its lowest-priority stream and runs the inverse FFT over the summed slots into the look-ahead ring, off
+ * the path of the real-time call.  Tail blocks need B >= 64.  Every shard gets the same input and call lengths (no input
+ * broadcast).  Staged handles with a sharded head (shard_head = 1) are refused: the fused exchange of those is for
+ * uniform (single-stage) handles only. */
 size_t b200conv_p2p_blob_size(const b200conv_t* h);
 int    b200conv_p2p_export(b200conv_t* h, void* blob, int mode);
 int    b200conv_p2p_import(b200conv_t* h, const void* all_blobs /* shard_count * blob_size bytes */);

@@ -33,7 +33,9 @@ class Engine:
     """C mono convolvers in one handle (b200conv_t)."""
 
     def __init__(self, n_channels: int = 1, device: int = 0, max_batch_blocks: int = 0,
-                 shard_rank: int = 0, shard_count: int = 1, cmac_variant: int = 0, lib=None):
+                 shard_rank: int = 0, shard_count: int = 1, cmac_variant: int = 0, lib=None, shard_head: bool = True):
+        """shard_head=False (sharded handles): rank 0 keeps the head stage whole and only the stages >= 1 are split
+        over the ranks — the real-time call stays one launch on rank 0 and no collective runs per call."""
         self._l = lib or _lib.default()
         cfg = _lib.Config(n_channels, device, max_batch_blocks, shard_rank, shard_count, cmac_variant)
         self._h = self._l.b200conv_create(C.byref(cfg))
@@ -41,6 +43,8 @@ class Engine:
             raise B200ConvError("b200conv_create failed")
         self.n_channels = n_channels
         self._reduce_cb = None
+        if not shard_head:
+            self.set_option("shard_head", 0)
 
     # -- helpers ---------------------------------------------------------------------------
     def _check(self, rc: int, what: str, allow_einval: bool = False) -> int:
@@ -251,7 +255,8 @@ class Engine:
         return int(self._l.b200conv_stream(self._h) or 0)
 
     def set_option(self, name: str, value: int):
-        """A/B switches of the engine: "rt" (one-launch real-time path), "fft512" (register-resident B = 512 FFTs), "tc" (tensor-core sweep for long launch groups)."""
+        """A/B switches of the engine: "rt" (one-launch real-time path), "fft512" (register-resident B = 512 FFTs), "tc" (tensor-core sweep for long launch groups);
+        "shard_head" (layout of a sharded handle, before the IR is loaded)."""
         self._check(self._l.b200conv_set_option(self._h, name.encode(), int(value)), "set_option")
 
     def set_timing(self, on: bool):

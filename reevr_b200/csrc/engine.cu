@@ -215,6 +215,15 @@ struct b200conv {
   std::vector<void*> ipc_opened;
   b200conv_barrier_fn host_barrier = nullptr;
   void* host_barrier_user = nullptr;
+  // tail-stage sharding (option "shard_head" = 0): rank 0 holds the head stage whole, only the stages >= 1 are
+  // partition-range sharded; their partial spectra reach rank 0 through the reduce hook or the tail slot exchange
+  bool opt_shard_head = true;
+  bool p2p_tail = false;                    // tail slot exchange attached
+  float2* Tx[4] = {};                       // stage s >= 1: [2 parities][G slots][2 rows][C][B] (used on rank 0)
+  float2* peerTx0[4] = {};                  // rank 0's Tx (mapped)
+  unsigned int* ttick = nullptr;            // tickets + tile counter of the exchange sweep (tail_tick_words)
+  unsigned long long tx_blocks[4] = {};     // tail blocks exchanged per stage since the attach (flag epochs)
+  bool rt_tail_joined = false;              // the last real-time call waited for a tail block (and its barrier)
 };
 
 namespace {
@@ -274,6 +283,9 @@ void p2p_release(b200conv* h) {
   cudaFree(h->Yx[0]); cudaFree(h->Yx[1]); cudaFree(h->Hh); cudaFree(h->xout[0]); cudaFree(h->xout[1]); cudaFree(h->xflags);
   h->Yx[0] = h->Yx[1] = nullptr; h->Hh = nullptr; h->xout[0] = h->xout[1] = nullptr; h->xflags = nullptr;
   h->p2p_on = false; h->hidx = 0; h->bar_epoch = 0; h->in_epoch = 0; h->xgrp = 0; h->bcast_in = false;
+  for (int s = 0; s < 4; ++s) { cudaFree(h->Tx[s]); h->Tx[s] = h->peerTx0[s] = nullptr; h->tx_blocks[s] = 0; }
+  cudaFree(h->ttick); h->ttick = nullptr;
+  h->p2p_tail = false;
   for (int i = 0; i < 2; ++i) { if (h->ev_b1[i]) cudaEventDestroy(h->ev_b1[i]); h->ev_b1[i] = nullptr; }
 }
 
@@ -377,6 +389,16 @@ void launch_inv_l(const pc::InvParams& P, const FftGeom& g, cudaStream_t st) {
     else pc::k_inv_fft_ola<(1 << L), false, false><<<g.grid, g.block, g.smem, st>>>(P);
   }
 }
+// loads the FFT kernels of block size 2^L a tail block of the slot exchange launches (lazy module loading)
+template <int L>
+cudaError_t fft_preload() {
+  cudaFuncAttributes fa;
+  cudaError_t e = cudaFuncGetAttributes(&fa, pc::k_fwd_fft<(1 << L), true>);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, pc::k_fwd_fft<(1 << L), false>);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, pc::k_inv_fft_ola<(1 << L), true, true>);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, pc::k_inv_fft_ola<(1 << L), false, true>);
+  return e;
+}
 template <int L>
 bool fft_set_smem_attr() {
   const int kSmem = 200 * 1024;   // B = 4096: 48 KB table + 64 KB ping-pong buffers; B = 8192: 128 KB buffers
@@ -394,6 +416,8 @@ bool stream_set_smem_attr() {
   ok = ok && cudaFuncSetAttribute(pc::k_cmac_stream_tma<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * pc::kStreamStageBytes + 64) == cudaSuccess;
   ok = ok && cudaFuncSetAttribute(pc::k_cmac_stream_tma<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 6 * pc::kStreamStageBytes + 128) == cudaSuccess;
   ok = ok && cudaFuncSetAttribute(pc::k_cmac_stream_tma<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, 12 * pc::kStreamStageBytes + 256) == cudaSuccess;
+  ok = ok && cudaFuncSetAttribute(pc::k_cmac_stream_tma<6, pc::StreamXchParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, 6 * pc::kStreamStageBytes + 128) == cudaSuccess;
+  ok = ok && cudaFuncSetAttribute(pc::k_cmac_stream_tma<12, pc::StreamXchParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, 12 * pc::kStreamStageBytes + 256) == cudaSuccess;
   ok = ok && cudaFuncSetAttribute(pc::k_cmac_stream_tma_dyn<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 6 * pc::kStreamStageBytes + 256) == cudaSuccess;
   ok = ok && cudaFuncSetAttribute(pc::k_cmac_stream_tma_dyn<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, 12 * pc::kStreamStageBytes + 512) == cudaSuccess;
   return ok;
@@ -616,7 +640,23 @@ int launch_stream_tma_s(b200conv* h, const pc::StreamParams& S_, dim3 grid) {
   return 0;
 }
 
-int launch_cmac_stream_tma(b200conv* h, const pc::CmacParams& P, int C, int stages, int per_sm, bool dynamic = false, float skew = -1.0f) {
+// the same sweep with the tail slot exchange epilogue
+template <int S>
+int launch_stream_tma_xch_s(b200conv* h, const pc::StreamParams& S_, const pc::StreamXchParams& X, dim3 grid) {
+#if defined(PC_EMULATE)
+  pc::emu_cmac_stream_tma({(int)grid.x, (int)grid.y, (int)grid.z}, S_, &X);
+#else
+  const size_t smem = (size_t)S * pc::kStreamStageBytes + 16 * S;
+  pc::k_cmac_stream_tma<S, pc::StreamXchParams><<<grid, dim3(288, 1, 1), smem, h->s_launch>>>(S_, X);
+#endif
+  return 0;
+}
+
+// destination of the tail slot exchange epilogue (launch_cmac_stream_tma with xch != nullptr)
+struct TailXch { float2* dst; unsigned int* flag; unsigned int epoch; };
+
+int launch_cmac_stream_tma(b200conv* h, const pc::CmacParams& P, int C, int stages, int per_sm, bool dynamic = false, float skew = -1.0f,
+                           const TailXch* xch = nullptr) {
   pc::StreamParams S{};
   S.H = P.H; S.h_cstride = P.h_cstride;
   S.X = P.X; S.x_cstride = P.x_cstride; S.xrow0 = P.xrow0;
@@ -657,11 +697,17 @@ int launch_cmac_stream_tma(b200conv* h, const pc::CmacParams& P, int C, int stag
     return 0;
   }
   int id = timing_begin(h, kKindCmac);
-  switch (stages) {
-    case 2: launch_stream_tma_s<2>(h, S, grid); break;
-    case 6: launch_stream_tma_s<6>(h, S, grid); break;
-    case 12: launch_stream_tma_s<12>(h, S, grid); break;
-    default: launch_stream_tma_s<4>(h, S, grid); break;
+  if (xch) {
+    const pc::StreamXchParams X{xch->dst, h->ttick, xch->flag, xch->epoch};
+    if (stages == 12) launch_stream_tma_xch_s<12>(h, S, X, grid);
+    else launch_stream_tma_xch_s<6>(h, S, X, grid);
+  } else {
+    switch (stages) {
+      case 2: launch_stream_tma_s<2>(h, S, grid); break;
+      case 6: launch_stream_tma_s<6>(h, S, grid); break;
+      case 12: launch_stream_tma_s<12>(h, S, grid); break;
+      default: launch_stream_tma_s<4>(h, S, grid); break;
+    }
   }
   timing_end(h, id);
   h->launches++;
@@ -828,10 +874,22 @@ int launch_cmac(b200conv* h, const pc::CmacParams& P, int C) {
   return 0;
 }
 
+// the single-block sweep of a tail block whose partial spectrum goes to rank 0 through the slot exchange: the TMA
+// streaming form launch_cmac selects for nblocks == 1 (also for an empty partition range: the zero slot is published too)
+int launch_cmac_exchange(b200conv* h, const pc::CmacParams& P, int C, const TailXch& x) {
+  const size_t bytes = (size_t)P.Ppad * P.B * 16 * (size_t)C;
+  const bool resident = P.B < 512 || (P.B == 512 && bytes <= (size_t)32 << 20);
+  h->last_variant = resident ? 104 : 103;
+  return resident ? launch_cmac_stream_tma(h, P, C, 12, 1, false, -1.0f, &x) : launch_cmac_stream_tma(h, P, C, 6, 2, false, -1.0f, &x);
+}
+
 int set_device(b200conv* h) {
   CU_CHECK(h, cudaSetDevice(h->cfg.device));
   return 0;
 }
+
+// shard_head = 0 on a sharded handle: the head stage stays whole on rank 0, the stages >= 1 are sharded
+bool tail_layout(const b200conv* h) { return !h->opt_shard_head && h->cfg.shard_count > 1; }
 
 // ---- IR load -------------------------------------------------------------------------------
 size_t trimmed_len(const float* ir, size_t n) {
@@ -859,6 +917,10 @@ int build_stage(b200conv* h, Stage& s, const float* const* ir, const std::vector
   const int per = (s.P_full + G - 1) / G;
   s.p_begin = std::min(s.P_full, g * per);
   s.p_end = std::min(s.P_full, (g + 1) * per);
+  if (tail_layout(h) && &s == &h->stages.front()) {     // the head: whole on rank 0, nothing on the other ranks
+    s.p_begin = 0;
+    s.p_end = g == 0 ? s.P_full : 0;
+  }
   s.P = s.p_end - s.p_begin;
   s.Prows = round_up(std::max(s.P, 1), kPadP) + kDPre;
   s.hist = s.p_begin + round_up(std::max(s.P, 1), kPadP) + kDPre;
@@ -987,6 +1049,14 @@ int clear_state(b200conv* h) {
     CU_CHECK(h, cudaMemsetAsync(h->Hh, 0, (size_t)3 * h->cfg.shard_count * row * sizeof(float2), h->s_main));
     h->hidx = 0;
   }
+  // tail slot exchange: the summed overlap rows (slot 0, row 0, both parities) on rank 0.  The peers' rows 1 are
+  // overwritten by every block, their rows 0 stay zero; the flag epochs keep counting on every rank alike.
+  for (size_t si = 1; si < h->stages.size() && h->cfg.shard_rank == 0; ++si)
+    if (h->Tx[si]) {
+      const size_t row = (size_t)h->C * h->stages[si].B;
+      for (int par = 0; par < 2; ++par)
+        CU_CHECK(h, cudaMemsetAsync(h->Tx[si] + (size_t)par * h->cfg.shard_count * 2 * row, 0, row * sizeof(float2), h->s_main));
+    }
   return 0;
 }
 
@@ -1192,7 +1262,7 @@ int p2p_alloc(b200conv* h) {
 // after a host synchronisation: did a flag barrier give up waiting for a peer?
 int p2p_check(b200conv* h) {
 #if !defined(PC_EMULATE)
-  if (h->xflags && h->bar_epoch + h->in_epoch > 0) {
+  if (h->xflags && (h->bar_epoch + h->in_epoch > 0 || h->p2p_tail)) {
     unsigned int err = 0;
     CU_CHECK(h, cudaMemcpy(&err, h->xflags + 8, sizeof(err), cudaMemcpyDeviceToHost));
     if (err != 0) {
@@ -1206,6 +1276,17 @@ int p2p_check(b200conv* h) {
 #endif
   return 0;
 }
+
+#if !defined(PC_EMULATE)
+unsigned long long p2p_timeout_ns() {
+  static const unsigned long long timeout_ms = [] {
+    const char* e = std::getenv("B200CONV_P2P_TIMEOUT_MS");
+    const long long v = e ? std::atoll(e) : 0;
+    return (unsigned long long)(v > 0 ? v : 4000);       // default 4 s (every kernel of the exchange is pre-loaded at attach)
+  }();
+  return timeout_ms * 1000000ull;
+}
+#endif
 
 // bank 0: exchange barriers (flag words 0..7, issued on s_post); bank 1: "input landed" barriers (words 16..23)
 int p2p_barrier(b200conv* h, cudaStream_t st, int bank = 0) {
@@ -1228,14 +1309,7 @@ int p2p_barrier(b200conv* h, cudaStream_t st, int bank = 0) {
   bp.my_flags = h->xflags + 16 * bank;
   bp.error_word = h->xflags + 8;
   bp.rank = h->cfg.shard_rank; bp.G = h->cfg.shard_count; bp.epoch = epoch;
-  {
-    static const unsigned long long timeout_ms = [] {
-      const char* e = std::getenv("B200CONV_P2P_TIMEOUT_MS");
-      const long long v = e ? std::atoll(e) : 0;
-      return (unsigned long long)(v > 0 ? v : 4000);       // default 4 s (every kernel of the exchange is pre-loaded at attach)
-    }();
-    bp.timeout_ns = timeout_ms * 1000000ull;
-  }
+  bp.timeout_ns = p2p_timeout_ns();
   pc::k_p2p_barrier<<<1, 32, 0, st>>>(bp);
   h->launches++;
   CU_CHECK(h, cudaGetLastError());
@@ -1255,6 +1329,200 @@ int copy_rows_kernel(b200conv* h, float* dst, size_t dpitch, const float* src, s
   h->launches++;
   CU_CHECK(h, cudaGetLastError());
 #endif
+  return 0;
+}
+
+// ---- tail slot exchange (stages >= 1 of a tail-sharded handle) ------------------------------------------------------
+// Rank 0 owns, per tail stage, Tx = [2 parities][G slots][2 rows][C][B]: rank g stores the partial spectrum of a
+// block into row 1 of slot g of the block's parity (sweep epilogue, peer store) and raises its flag in the stage's
+// bank.  Row 0 of slot 0 is the summed spectrum of the previous block (the overlap state), rows 0 of the other slots
+// stay zero, so that the inverse FFT summing the G slots (n_partials = G) sees the full sums of both rows.  A slot is
+// written again two blocks later: rank g first waits until rank 0 has reached the barrier of the block in between,
+// which it issues after the inverse FFT that read the slot.
+constexpr int kFlagWords = 96;           // bank 0 words 0..7 + error word 8, bank 1 words 16..23, tail banks below
+int tail_bank(int si) { return 32 + 16 * (si - 1); }
+
+// ticket words of the exchange sweep: one per (channel, bin tile) of the widest tail stage (its grid is
+// B / stream_tma_w(B) x nsplit x C) + the tile counter
+size_t tail_tick_words(const b200conv* h) {
+  int tiles = 1;
+  for (size_t si = 1; si < h->stages.size(); ++si) tiles = std::max(tiles, h->stages[si].B / pc::stream_tma_w(h->stages[si].B));
+  return (size_t)h->C * tiles + 1;
+}
+
+int p2p_alloc_tail(b200conv* h) {
+  if (h->ttick) return 0;
+  const int G = h->cfg.shard_count, C = h->C;
+  CU_CHECK(h, cudaMalloc(&h->xflags, kFlagWords * sizeof(unsigned int)));
+  CU_CHECK(h, cudaMemsetAsync(h->xflags, 0, kFlagWords * sizeof(unsigned int), h->s_main));
+  const size_t ticks = tail_tick_words(h);
+  CU_CHECK(h, cudaMalloc(&h->ttick, ticks * sizeof(unsigned int)));
+  CU_CHECK(h, cudaMemsetAsync(h->ttick, 0, ticks * sizeof(unsigned int), h->s_main));
+  for (size_t si = 1; si < h->stages.size() && h->cfg.shard_rank == 0; ++si) {
+    const size_t bytes = (size_t)2 * G * 2 * C * h->stages[si].B * sizeof(float2);
+    CU_CHECK(h, cudaMalloc(&h->Tx[si], bytes));
+    CU_CHECK(h, cudaMemsetAsync(h->Tx[si], 0, bytes, h->s_main));
+  }
+#if !defined(PC_EMULATE)
+  // every kernel a tail block launches, loaded now (see p2p_alloc)
+  {
+    cudaFuncAttributes fa;
+    CU_CHECK(h, cudaFuncGetAttributes(&fa, pc::k_p2p_barrier));
+    CU_CHECK(h, cudaFuncGetAttributes(&fa, pc::k_sum_slots));
+    CU_CHECK(h, cudaFuncGetAttributes(&fa, pc::k_cmac_stream_tma<6, pc::StreamXchParams>));
+    CU_CHECK(h, cudaFuncGetAttributes(&fa, pc::k_cmac_stream_tma<12, pc::StreamXchParams>));
+    CU_CHECK(h, cudaFuncGetAttributes(&fa, pc::k_fwd_fft512));
+    for (size_t si = 1; si < h->stages.size(); ++si) {
+      cudaError_t e = cudaErrorInvalidValue;
+      switch (pc::ilog2(h->stages[si].B)) {
+#define PC_CASE(L) case L: e = fft_preload<L>(); break;
+        PC_FOR_EACH_LOG2(PC_CASE)
+#undef PC_CASE
+        default: break;
+      }
+      CU_CHECK(h, e);
+    }
+  }
+#endif
+  CU_CHECK(h, cudaStreamSynchronize(h->s_main));
+  return 0;
+}
+
+// host-side rendezvous of all shards (emulation build, shards sharing one device in one process)
+int host_rendezvous(b200conv* h, cudaStream_t st) {
+  CU_CHECK(h, cudaStreamSynchronize(st));
+  if (h->host_barrier(h->host_barrier_user) != 0) return fail(h, B200CONV_ECUDA, "host barrier failed");
+  return 0;
+}
+
+// rank 0: every rank's flag of block e is up (it publishes e in the peers' banks first); rank g >= 1: rank 0 has
+// published e (this waits only: the scratch word 8 of the bank takes the publish)
+int tail_flag_wait(b200conv* h, cudaStream_t st, int si, unsigned int e) {
+#if defined(PC_EMULATE)
+  (void)st; (void)si; (void)e;
+  return fail(h, B200CONV_ESTATE, "emulated slot exchange needs a host barrier");
+#else
+  const int off = tail_bank(si);
+  pc::BarrierParams bp{};
+  bp.my_flags = h->xflags + off;
+  bp.error_word = h->xflags + 8;
+  bp.rank = 0; bp.epoch = e;
+  bp.timeout_ns = p2p_timeout_ns();
+  if (h->cfg.shard_rank == 0) {
+    bp.G = h->cfg.shard_count;
+    for (int g = 0; g < bp.G; ++g) bp.peer_flags[g] = h->peer_flags[g] + off;
+  } else {
+    bp.G = 1;
+    bp.peer_flags[0] = h->xflags + off + 8;
+  }
+  pc::k_p2p_barrier<<<1, 32, 0, st>>>(bp);
+  h->launches++;
+  CU_CHECK(h, cudaGetLastError());
+  return 0;
+#endif
+}
+
+int launch_sum_slots(b200conv* h, float2* dst, const float2* src, size_t n, int np, size_t ps, cudaStream_t st) {
+#if defined(PC_EMULATE)
+  (void)h; (void)st;
+  for (size_t i = 0; i < n; ++i) dst[i] = pc::sum_partials(src + i, 0, np, (long long)ps);
+#else
+  pc::k_sum_slots<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(dst, src, (long long)n, np, (long long)ps);
+  h->launches++;
+  CU_CHECK(h, cudaGetLastError());
+#endif
+  return 0;
+}
+
+// One completed block of a stage >= 1 of a tail-sharded handle, spectrum in X row s.head (output block s.blocks_done),
+// everything on h->s_launch: the sweep over this rank's partitions, the partial spectra of all ranks summed on rank 0
+// (slot exchange, else the reduce hook), and on rank 0 the inverse FFT into the stage's look-ahead ring.
+int tail_block(b200conv* h, Stage& s, int si) {
+  const int C = h->C, B = s.B, G = h->cfg.shard_count, g = h->cfg.shard_rank;
+  const size_t row = (size_t)C * B;
+  cudaStream_t st = h->s_launch;
+  float2* Yb = s.Y[s.ybuf];
+  pc::CmacParams cp{};
+  cp.H = s.H; cp.h_cstride = (long long)s.Prows * B;
+  cp.X = s.X; cp.x_cstride = (long long)s.R * B; cp.xrow0 = s.head - s.p_begin;
+  cp.Y = Yb; cp.y_cstride = B; cp.y_rstride = (long long)row; cp.yrow0 = 1;
+  cp.B = B; cp.Ppad = s.P; cp.nblocks = 1;
+  pc::InvParams ip{};
+  ip.y_cstride = B; ip.y_rstride = (long long)row; ip.yrow0 = 1;
+  ip.tw = s.tw; ip.tab512 = s.tab512; ip.M = B; ip.nblocks = 1; ip.scale = 1.0f / (float)B;
+  ip.dst = s.fut; ip.dst_cstride = (long long)s.ring;
+  ip.index0 = (s.blocks_done + s.q) * (long long)B;
+  ip.lo = 0; ip.hi = (long long)1 << 62; ip.mask = (long long)s.ring - 1;
+  if (!h->p2p_tail) {                       // reduce hook: once per tail block, never for the head
+    if (s.P > 0) { if (int rc = launch_cmac(h, cp, C)) return rc; }
+    else CU_CHECK(h, cudaMemsetAsync(Yb + row, 0, row * sizeof(float2), st));
+    if (!h->reduce) return fail(h, B200CONV_ESTATE, "sharded handle without a reduce hook");
+    if (h->reduce(h->reduce_user, reinterpret_cast<float*>(Yb + row), row * 2, st) != 0)
+      return fail(h, B200CONV_ECUDA, "reduce hook failed");
+    if (g == 0) {
+      ip.Y = Yb;
+      if (int rc = launch_inv(h, ip, C, st)) return rc;
+      CU_CHECK(h, cudaMemcpyAsync(Yb, Yb + row, row * sizeof(float2), cudaMemcpyDeviceToDevice, st));   // overlap state
+    }
+    return 0;
+  }
+  const unsigned long long e = ++h->tx_blocks[si];
+  const size_t par = (size_t)G * 2 * row;                      // float2 per parity
+  if (g > 0 && !h->host_barrier && e > 1) { if (int rc = tail_flag_wait(h, st, si, (unsigned int)(e - 1))) return rc; }
+  const TailXch x{h->peerTx0[si] + (size_t)(e & 1) * par + (size_t)g * 2 * row + row,
+                  h->peer_flags[0] + tail_bank(si) + g, (unsigned int)e};
+  if (int rc = launch_cmac_exchange(h, cp, C, x)) return rc;
+  if (h->host_barrier) { if (int rc = host_rendezvous(h, st)) return rc; }
+  else if (g == 0) { if (int rc = tail_flag_wait(h, st, si, (unsigned int)e)) return rc; }
+  if (g == 0) {
+    float2* mine = h->Tx[si] + (size_t)(e & 1) * par;
+    ip.Y = mine; ip.n_partials = G; ip.partial_stride = (long long)(2 * row);
+    if (int rc = launch_inv(h, ip, C, st)) return rc;
+    // the summed spectrum -> overlap row of the next block (the other parity)
+    if (int rc = launch_sum_slots(h, h->Tx[si] + (size_t)((e + 1) & 1) * par, mine + row, row, G, 2 * row, st)) return rc;
+  }
+  return 0;
+}
+
+// Stages >= 1 of a tail-sharded handle for one launch group of n samples: forward FFT of the completed blocks, then
+// tail_block for each, stage by stage in ascending order (the same sequence of exchanges / hook calls on every rank
+// and on every path, the real-time one included).
+int run_tail_stages(b200conv* h, const float* in_dev, size_t in_stride, size_t n) {
+  const int C = h->C;
+  for (size_t si = 1; si < h->stages.size(); ++si) {
+    Stage& s = h->stages[si];
+    const int B = s.B;
+    const size_t total = (size_t)s.fill + n;
+    const int complete = (int)(total / B);
+    const int partial = (int)(total % B);
+    const bool direct = (s.fill == 0);
+    if (!direct) { if (int rc = copy_in(h, s.inbuf + s.fill, s.in_stride, in_dev, in_stride, n)) return rc; }
+    if (complete > 0) {
+      if (s.head + complete + kMaxTT > s.R) { if (int rc = compact_timeline(h, s)) return rc; }
+      pc::FwdParams fp{};
+      fp.src = direct ? in_dev : s.inbuf;
+      fp.src_cstride = direct ? (long long)in_stride : (long long)s.in_stride;
+      fp.nvalid_c = nullptr; fp.nvalid = (long long)total;
+      set_cmap(h, fp, direct);
+      fp.dst = s.X; fp.dst_cstride = (long long)s.R * B; fp.dst_row0 = s.head;
+      fp.tw = s.tw; fp.tab512 = s.tab512; fp.M = B; fp.nblocks = complete;
+      if (int rc = launch_fwd(h, fp, C)) return rc;
+      for (int j = 0; j < complete; ++j) {
+        if (int rc = tail_block(h, s, (int)si)) return rc;
+        s.head += 1;
+        s.blocks_done += 1;
+      }
+      if (partial > 0) {
+        if (direct) { if (int rc = copy_in(h, s.inbuf, s.in_stride, in_dev + (size_t)complete * B, in_stride, partial)) return rc; }
+        else
+          CU_CHECK(h, cudaMemcpy2DAsync(s.inbuf, s.in_stride * sizeof(float), s.inbuf + (size_t)complete * B,
+                                        s.in_stride * sizeof(float), partial * sizeof(float), C, cudaMemcpyDeviceToDevice, h->s_main));
+      }
+    } else if (direct && partial > 0) {
+      if (int rc = copy_in(h, s.inbuf, s.in_stride, in_dev, in_stride, partial)) return rc;
+    }
+    s.fill = partial;
+  }
   return 0;
 }
 
@@ -1347,6 +1615,7 @@ int run_group_p2p(b200conv* h, const float* in_dev, size_t in_stride, float* out
 }
 
 int drain_tail(b200conv* h);
+int join_post(b200conv* h);
 
 // `overlap`: reduce + inverse FFT go to s_post so that they overlap the next group's forward
 // FFT + sweep on s_main (double-buffered Y); otherwise everything is issued on s_main.
@@ -1362,8 +1631,15 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
   if (n == 0) return 0;
   if (n + h->stages[0].B > h->Lmax) return fail(h, B200CONV_ESTATE, "launch group larger than the staging buffers");
   if (int rc = drain_tail(h)) return rc;
+  const bool tails = tail_layout(h);
+  if (tails) {
+    // stages >= 1 block by block on s_main, behind the previous group's head output (which reads their rings)
+    if (overlap) { if (int rc = join_post(h)) return rc; }
+    if (int rc = run_tail_stages(h, in_dev, in_stride, n)) return rc;
+    if (!root) { h->abs_pos += (long long)n; return 0; }     // no head partitions on this rank
+  }
   // stages >= 1 first (their look-ahead output may be consumed by the head within this group)
-  for (int si = (int)h->stages.size() - 1; si >= 0; --si) {
+  for (int si = tails ? 0 : (int)h->stages.size() - 1; si >= 0; --si) {
     Stage& s = h->stages[si];
     const int B = s.B;
     const size_t row = (size_t)C * B;           // float2 per Y row (all channels)
@@ -1409,7 +1685,7 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
         CU_CHECK(h, cudaStreamWaitEvent(ps, s.ev_sweep[yb], 0));
       }
 
-      if (h->cfg.shard_count > 1) {
+      if (h->cfg.shard_count > 1 && !tails) {
         if (!h->reduce) return fail(h, B200CONV_ESTATE, "sharded handle without a reduce hook");
         if (h->reduce(h->reduce_user, reinterpret_cast<float*>(Yb + row), (size_t)nb * row * 2, ps) != 0)
           return fail(h, B200CONV_ECUDA, "reduce hook failed");
@@ -1547,6 +1823,13 @@ int run_tail_block(b200conv* h, Stage& s) {
   fp.dst = s.X; fp.dst_cstride = (long long)s.R * B; fp.dst_row0 = s.head;
   fp.tw = s.tw; fp.tab512 = s.tab512; fp.M = B; fp.nblocks = 1;
   if (int rc = launch_fwd(h, fp, C)) return rc;
+  if (tail_layout(h)) {            // rank 0 of a tail-sharded handle: the other ranks' partial spectra join here
+    if (int rc = tail_block(h, s, (int)(&s - h->stages.data()))) return rc;
+    s.head += 1;
+    s.blocks_done += 1;
+    s.fill = 0;
+    return 0;
+  }
   float2* Yb = s.Y[s.ybuf];
   pc::CmacParams cp{};
   cp.H = s.H; cp.h_cstride = (long long)s.Prows * B;
@@ -1574,7 +1857,9 @@ constexpr size_t kRtMaxBytesPerCta = 384 * 1024;      // H + FDL bytes one CTA o
 // CTAs per convolver for the cluster kernel; -1 = split mode (head stage too large for one cluster); 0 = the call does not qualify
 int rt_cluster_ctas(const b200conv* h, size_t len) {
   if (!h->opt_rt || h->stages.empty() || h->stages.size() > 4) return 0;
-  if (h->cfg.shard_count != 1 || h->p2p_on || h->timing || h->yprev_stale) return 0;
+  // rank 0 of a tail-sharded handle holds the head whole: its tail blocks are exchanged by run_tail_block
+  const bool whole_head = h->cfg.shard_count == 1 || (tail_layout(h) && h->cfg.shard_rank == 0);
+  if (!whole_head || h->p2p_on || h->timing || h->yprev_stale) return 0;
   const Stage& s0 = h->stages[0];
   const int M = s0.B, C = h->C;
   if (M < 16 || M > 1024 || C > 8 || len == 0 || (size_t)s0.fill + len > (size_t)M) return 0;
@@ -1626,6 +1911,7 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
       if (!s.job_waited[j] && h->abs_pos + (long long)len > s.job_out_start[j]) {
         CU_CHECK(h, cudaStreamWaitEvent(h->s_main, s.ev_job[j], 0));
         s.job_waited[j] = true;
+        h->rt_tail_joined = true;
       }
   }
   if (s0.head + 1 + kMaxTT > s0.R) { if (int rc = compact_timeline(h, s0)) return rc; }
@@ -2064,6 +2350,10 @@ static int process_impl(b200conv_t* h, const float* const* in, float* const* out
       if (!done) CU_CHECK(h, cudaStreamSynchronize(h->s_main));
       if (out)
         for (int c = 0; c < Cout; ++c) std::memcpy(out[c], h->hpin_out + (size_t)c * len, len * sizeof(float));
+      if (h->p2p_tail && h->rt_tail_joined) {     // a tail block's barrier has run: did it give up on a peer?
+        h->rt_tail_joined = false;
+        return p2p_check(h);
+      }
       return B200CONV_OK;
     }
     // latency path: one stream, one group; all channels travel in ONE pinned H2D and ONE D2H copy
@@ -2755,6 +3045,10 @@ int b200conv_set_option(b200conv_t* h, const char* name, int value) {
   else if (n == "slice_keep_tail") h->opt_slice_tail = value != 0;
   else if (n == "stream_alternate") h->opt_stream_alt = value != 0;
   else if (n == "tc") h->opt_tc = value != 0;
+  else if (n == "shard_head") {
+    if (!h->stages.empty()) return fail(h, B200CONV_ESTATE, "shard_head is set before the impulse response is loaded");
+    h->opt_shard_head = value != 0;
+  }
   else return fail(h, B200CONV_EINVAL, "unknown option");
   return B200CONV_OK;
 }
@@ -2824,11 +3118,20 @@ int b200conv_p2p_import(b200conv_t* h, const void* all_blobs) {
 static int p2p_export_impl(b200conv_t* h, void* blob, int mode) {
   if (!blob) return fail(h, B200CONV_EINVAL, "null blob");
   if (h->cfg.shard_count < 2 || h->cfg.shard_count > 8) return fail(h, B200CONV_ESTATE, "slot exchange needs 2..8 shards");
-  if (h->stages.size() != 1) return fail(h, B200CONV_ESTATE, "slot exchange supports uniform (single-stage) handles");
+  const bool tails = tail_layout(h);
+  if (tails) {
+    if (h->stages.empty()) return fail(h, B200CONV_ESTATE, "load an impulse response first");
+    for (size_t si = 1; si < h->stages.size(); ++si)
+      if (h->stages[si].B < 64) return fail(h, B200CONV_ESTATE, "the tail slot exchange needs tail blocks of at least 64 samples");
+  } else if (h->stages.size() != 1) {
+    return fail(h, B200CONV_ESTATE, "slot exchange supports uniform (single-stage) handles, or staged handles with shard_head = 0");
+  }
   if (int rc = set_device(h)) return rc;
-  if (int rc = p2p_alloc(h)) return rc;
+  if (int rc = tails ? p2p_alloc_tail(h) : p2p_alloc(h)) return rc;
   h->p2p_mode = mode;
+  // tail layout: records 0..2 = Tx of stages 1..3 (rank 0 only), 5 = flags; the others stay empty
   void* bufs[kP2PBuffers] = {h->Yx[0], h->Yx[1], h->Hh, h->xout[0], h->xout[1], h->xflags, h->din[0], h->din[1]};
+  if (tails) for (int i = 0; i < kP2PBuffers; ++i) bufs[i] = i < 3 ? (void*)h->Tx[i + 1] : (i == 5 ? (void*)h->xflags : nullptr);
   P2PRecord* rec = static_cast<P2PRecord*>(blob);
   for (int i = 0; i < kP2PBuffers; ++i) {
     std::memset(&rec[i], 0, sizeof(P2PRecord));
@@ -2836,7 +3139,7 @@ static int p2p_export_impl(b200conv_t* h, void* blob, int mode) {
 #if defined(PC_EMULATE)
     rec[i].kind = 1;
 #else
-    if (mode == 1) {
+    if (mode == 1 || !bufs[i]) {
       rec[i].kind = 1;
     } else {
       rec[i].kind = 2;
@@ -2850,7 +3153,47 @@ static int p2p_export_impl(b200conv_t* h, void* blob, int mode) {
   return B200CONV_OK;
 }
 
+static int p2p_import_tail(b200conv_t* h, const void* all_blobs) {
+  const int G = h->cfg.shard_count, me = h->cfg.shard_rank;
+  const P2PRecord* rec = static_cast<const P2PRecord*>(all_blobs);
+  for (int r = 0; r < G; ++r)
+    for (int i = 0; i < kP2PBuffers; ++i) {
+      const P2PRecord& x = rec[r * kP2PBuffers + i];
+      // every rank's flags (rank 0 publishes into them), rank 0's Tx (every rank stores its slots there)
+      if (!(i == 5 || (r == 0 && i < 3))) continue;
+      void* p = (void*)(uintptr_t)x.ptr;
+      if (r != me && x.kind != 1) {
+#if defined(PC_EMULATE)
+        return fail(h, B200CONV_EINVAL, "IPC records in the emulation build");
+#else
+        cudaIpcMemHandle_t hd;
+        std::memcpy(&hd, x.ipc, 64);
+        CU_CHECK(h, cudaIpcOpenMemHandle(&p, hd, cudaIpcMemLazyEnablePeerAccess));
+        h->ipc_opened.push_back(p);
+#endif
+      }
+      if (i == 5) h->peer_flags[r] = static_cast<unsigned int*>(p);
+      else h->peerTx0[i + 1] = static_cast<float2*>(p);
+    }
+  // rank 0 keeps the overlap state of every tail stage in its Tx from now on (the reduce-hook path kept it in Y row 0)
+  CU_CHECK(h, cudaStreamSynchronize(h->s_tail));
+  CU_CHECK(h, cudaStreamSynchronize(h->s_post));
+  for (size_t si = 1; si < h->stages.size() && me == 0; ++si) {
+    const Stage& s = h->stages[si];
+    const size_t row = (size_t)h->C * s.B;
+    CU_CHECK(h, cudaMemcpyAsync(h->Tx[si] + (size_t)((h->tx_blocks[si] + 1) & 1) * G * 2 * row, s.Y[s.ybuf],
+                                row * sizeof(float2), cudaMemcpyDeviceToDevice, h->s_main));
+  }
+  CU_CHECK(h, cudaStreamSynchronize(h->s_main));
+  h->p2p_tail = true;
+  return B200CONV_OK;
+}
+
 static int p2p_import_impl(b200conv_t* h, const void* all_blobs) {
+  if (all_blobs && h->ttick) {
+    if (int rc = set_device(h)) return rc;
+    return p2p_import_tail(h, all_blobs);
+  }
   if (!all_blobs || !h->Yx[0]) return fail(h, B200CONV_ESTATE, "export before import");
   if (int rc = set_device(h)) return rc;
   const int G = h->cfg.shard_count, me = h->cfg.shard_rank;
@@ -2924,8 +3267,20 @@ int b200conv_p2p_set_input_broadcast(b200conv_t* h, int enable) {
 int b200conv_p2p_detach(b200conv_t* h) {
   if (!h) return B200CONV_EINVAL;
   if (h->s_main) { cudaSetDevice(h->cfg.device); cudaStreamSynchronize(h->s_main); if (h->s_post) cudaStreamSynchronize(h->s_post); }
+  if (h->p2p_tail && !h->sticky_cuda_error && h->cfg.shard_rank == 0) {
+    // the reduce-hook path takes the overlap state of every tail stage back into Y row 0
+    CU_CHECK(h, cudaStreamSynchronize(h->s_tail));
+    for (size_t si = 1; si < h->stages.size(); ++si) {
+      const Stage& s = h->stages[si];
+      const size_t row = (size_t)h->C * s.B;
+      CU_CHECK(h, cudaMemcpyAsync(s.Y[s.ybuf], h->Tx[si] + (size_t)((h->tx_blocks[si] + 1) & 1) * h->cfg.shard_count * 2 * row,
+                                  row * sizeof(float2), cudaMemcpyDeviceToDevice, h->s_main));
+    }
+    CU_CHECK(h, cudaStreamSynchronize(h->s_main));
+  }
   const int rc = h->sticky_cuda_error ? B200CONV_OK : p2p_check(h);   // a barrier that gave up is reported here at the latest
   h->p2p_on = false;
+  h->p2p_tail = false;
   h->bcast_in = false;
   return rc;
 }

@@ -621,6 +621,17 @@ struct StreamParams {
   int descending;
 };
 
+// tail slot exchange epilogue of k_cmac_stream_tma (its optional second parameter): the last CTA of every (bin tile,
+// channel) stores the summed tile into xdst (this rank's slot on rank 0, peer memory, channel pitch y_cstride); the last
+// tile of the launch raises *xflag = xepoch.  xtick: one ticket word per (channel, bin tile) + one tile counter, zero
+// between launches.
+struct StreamXchParams {
+  float2* xdst;
+  unsigned int* xtick;
+  unsigned int* xflag;
+  unsigned int xepoch;
+};
+
 #if defined(__CUDACC__)
 // ==========================================================================================
 // __global__ wrappers
@@ -965,6 +976,13 @@ static __global__ void k_copy_rows(float* dst, long long dpitch, const float* sr
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const int r = blockIdx.y;
   if (i < width && r < rows) dst[(long long)r * dpitch + i] = src[(long long)r * spitch + i];
+}
+
+// dst[i] = sum over np slots of src[g*ps + i] (tail slot exchange: the summed spectrum of a tail block becomes the
+// overlap row of the next one); same summation order as the inverse FFT's sum_partials
+static __global__ void k_sum_slots(float2* dst, const float2* src, long long n, int np, long long ps) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = sum_partials(src + i, 0, np, ps);
 }
 #endif  // __CUDACC__
 

@@ -121,9 +121,17 @@ PC_D void bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long lon
                ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
-// grid (B / W, nsplit, C), block 288 = 8 consumer warps + 1 producer warp; dynamic smem = S*16 KB + 16*S bytes
-template <int S>
-__global__ void __launch_bounds__(288) k_cmac_stream_tma(StreamParams P) {
+// grid (B / W, nsplit, C), block 288 = 8 consumer warps + 1 producer warp; dynamic smem = S*16 KB + 16*S bytes.
+// With a StreamXchParams argument (Xch = StreamXchParams): the tail slot exchange epilogue.  A tile's value is final
+// only once the last of its nsplit CTAs has added its share, so every CTA (empty slices included) takes a ticket of its
+// (channel, bin tile) after a release fence; the CTA drawing the last one reads the summed tile back from L2 and stores
+// it into this rank's slot on rank 0, then counts the tile; the last tile raises this rank's flag with a system-scope
+// release.  Without it (empty pack) the kernel and its parameter block are exactly the plain sweep's.
+template <class T> PC_D const T& stream_xch_arg(const T& x) { return x; }
+
+template <int S, class... Xch>
+__global__ void __launch_bounds__(288) k_cmac_stream_tma(StreamParams P, Xch... xch) {
+  constexpr bool XCH = sizeof...(Xch) > 0;
   extern __shared__ __align__(128) unsigned char pc_stream_smem[];
   float2* ring = reinterpret_cast<float2*>(pc_stream_smem);
   unsigned long long* full = reinterpret_cast<unsigned long long*>(pc_stream_smem + (size_t)S * kStreamStageBytes);
@@ -139,7 +147,10 @@ __global__ void __launch_bounds__(288) k_cmac_stream_tma(StreamParams P) {
   } else {
     stream_slice(P.P, P.nsplit, blockIdx.y, &p_lo, &p_hi);
   }
-  if (p_lo >= p_hi) return;                                  // whole CTA (uniform)
+  if (p_lo >= p_hi) {                                        // whole CTA (uniform)
+    if constexpr (!XCH) return;
+    else p_hi = p_lo;                                        // no stage, but the CTA still takes its ticket
+  }
   const int nst = (p_hi - p_lo + PP - 1) / PP;
   if (tid == 0) {
     for (int s = 0; s < S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
@@ -190,10 +201,42 @@ __global__ void __launch_bounds__(288) k_cmac_stream_tma(StreamParams P) {
     atomicAdd(y + 0, acc[0].x); atomicAdd(y + 1, acc[0].y);
     atomicAdd(y + 2, acc[1].x); atomicAdd(y + 3, acc[1].y);
   }
+  if constexpr (XCH) {
+    const StreamXchParams& X = stream_xch_arg(xch...);
+    // the 256 consumer threads only (named barrier 1): the producer warp has left
+    int* last = reinterpret_cast<int*>(pc_stream_smem);       // stage 0 is free: every stage has been consumed
+    __threadfence();
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (tid == 0) {
+      __threadfence();
+      unsigned int* tick = X.xtick + (size_t)c * gridDim.x + blockIdx.x;
+      const bool is_last = atomicAdd(tick, 1u) == gridDim.y - 1;
+      if (is_last) { *tick = 0; __threadfence(); }
+      *last = is_last ? 1 : 0;
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (*last) {
+      if (rg == 0) {
+        const float4 v = __ldcg(reinterpret_cast<const float4*>(y));
+        *reinterpret_cast<float4*>(X.xdst + (long long)c * P.y_cstride + k0 + 2 * col) = v;
+      }
+      __threadfence_system();
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (tid == 0) {
+        unsigned int* tiles = X.xtick + (size_t)gridDim.x * gridDim.z;
+        __threadfence_system();
+        if (atomicAdd(tiles, 1u) == gridDim.x * gridDim.z - 1) {
+          *tiles = 0;
+          __threadfence_system();
+          asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(X.xflag), "r"(X.xepoch) : "memory");
+        }
+      }
+    }
+  }
 }
 #else
 // CPU emulation (tests/emu): same slices, stages and consumer arithmetic; memcpy stands in for the bulk copies
-inline void emu_cmac_stream_tma(EmuDim grid, const StreamParams& P) {
+inline void emu_cmac_stream_tma(EmuDim grid, const StreamParams& P, const StreamXchParams* X = nullptr) {
   const int W = stream_tma_w(P.B), PP = stream_tma_pp(P.B), RG = stream_tma_rg(P.B);
   float2* stage = new float2[kStreamStageBytes / 8];
   for (int cz = 0; cz < grid.z; ++cz)
@@ -239,6 +282,12 @@ inline void emu_cmac_stream_tma(EmuDim grid, const StreamParams& P) {
         delete[] accs;
       }
   delete[] stage;
+  if (X) {                      // tail slot exchange epilogue: every tile is final here
+    for (int c = 0; c < grid.z; ++c)
+      std::memcpy(X->xdst + (long long)c * P.y_cstride, P.Y + (long long)c * P.y_cstride + P.yrow0 * P.y_rstride,
+                  (size_t)P.B * sizeof(float2));
+    *X->xflag = X->xepoch;
+  }
 }
 #endif
 

@@ -7,6 +7,11 @@ engine calls back into `attach_reduce`'s hook, which sums the partial spectra of
 rank 0 with ONE collective per launch group (ncclReduce over NVLink under the "nccl" backend).
 Only rank 0 runs the inverse FFT / overlap-add and produces audio.
 
+Tail layout (Engine(..., shard_head=False)): rank 0 keeps the head stage whole and only the stages >= 1 are split.
+The hook then runs once per completed tail block (never for the head), and `attach_p2p` attaches the tail slot
+exchange instead: every rank stores its partial tail spectrum into rank 0's slots over peer memory, off the path of the
+real-time call.
+
 The "gloo" branch exists for the world_size-2 CPU tests: with the emulation build of the C ABI
 the "device" pointers are host memory, so the same hook reduces them with gloo.
 """
@@ -53,7 +58,8 @@ def attach_reduce(engine, device: int | None = None, group=None, root: int = 0) 
 
 
 def attach_p2p(engine, group=None) -> tuple:
-    """Enables the fused slot-exchange path on a sharded uniform Engine.  torch.distributed only moves the
+    """Enables the fused slot-exchange path on a sharded uniform Engine, or the tail slot exchange on an Engine created
+    with shard_head=False (any stage schedule).  torch.distributed only moves the
     CUDA IPC blobs (plumbing) — the data path makes no NCCL call.  Every rank executes the same collectives
     whether or not its own export / import works, and all ranks end on the SAME path:
     returns (True, "") if the exchange is active everywhere, else (False, reason) with the exchange detached."""
