@@ -114,7 +114,7 @@ size_t b200conv_ir_len(const b200conv_t* h, int channel);    /* post-trim tap co
 /* Kernel launches issued by this handle since creation (bench.py's gpu_launches). */
 unsigned long long b200conv_launch_count(const b200conv_t* h);
 /* Form of the FDL sweep (FFTConvolver.cpp:176-187) the last launch resolved to: 22 / 26 = packed-FMA batched sweep,
- * 40 = tensor-core sweep (wgmma tf32, 3xTF32), 100..108 = streaming forms.  For benchmarks and tests. */
+ * 40 = tensor-core sweep (wgmma f16, 3xFP16 with power-of-two scales), 100..108 = streaming forms.  For benchmarks and tests. */
 int b200conv_last_sweep_variant(const b200conv_t* h);
 /* Tuning / A-B switches: "rt" (1 = real-time calls that stay inside the open block run as ONE cluster-kernel launch
  * with zero-copy I/O, 0 = multi-kernel path), "fft512" (1 = register-resident FFT kernels for block size 512),

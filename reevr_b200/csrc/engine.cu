@@ -180,7 +180,7 @@ struct b200conv {
   bool opt_slice_tail = true;        // sliced calls: also transform the last P blocks of the call (full-state contract)
   // tensor-core sweep (kernels_tc.cuh): Toeplitz tile images of one stage's H, per-bin time lines, partial planes
   bool opt_tc = std::getenv("B200CONV_NO_TC") == nullptr;
-  float* tc_A = nullptr;
+  void* tc_A = nullptr;              // FP16 images, then the per-line scale exponents (kernels_tc.cuh a_image_bytes)
   const void* tc_A_for = nullptr;    // H the images were built from (+ its geometry)
   int tc_A_P = 0, tc_A_B = 0, tc_A_C = 0;
   float* tc_Xt = nullptr;
@@ -733,11 +733,12 @@ bool tc_eligible(const b200conv* h, const pc::CmacParams& P, int C) {
 
 #if !defined(PC_EMULATE)
 // grow-only device scratch; a failed allocation is not an error of the call (the caller falls back to the FFMA sweep)
-bool tc_reserve(b200conv* h, float** buf, size_t* have, size_t need) {
+template <typename T>
+bool tc_reserve(b200conv* h, T** buf, size_t* have, size_t need) {
   if (*have >= need) return true;
   cudaFree(*buf);
   *buf = nullptr; *have = 0;
-  if (cudaMalloc(buf, need) != cudaSuccess) { cudaGetLastError(); *buf = nullptr; h->tc_alloc_failed = true; return false; }
+  if (cudaMalloc((void**)buf, need) != cudaSuccess) { cudaGetLastError(); *buf = nullptr; h->tc_alloc_failed = true; return false; }
   *have = need;
   return true;
 }
@@ -759,31 +760,34 @@ int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C) {
   }
   if (*reinterpret_cast<volatile int*>(h->tc_err) != 0)
     return fail(h, B200CONV_ECUDA, "tensor-core sweep: a pipeline barrier timed out (code " + std::to_string(*h->tc_err) + ")");
-  if (!tc_reserve(h, &h->tc_Xt, &h->tc_Xt_bytes, lines * 4 * (size_t)g.Lt * sizeof(float))) return 1;
+  const int nchunk = tc::nchunk_f16(g.Q);
+  if (!tc_reserve(h, &h->tc_Xt, &h->tc_Xt_bytes, lines * 2 * (size_t)g.Lt * sizeof(float))) return 1;
   if (!tc_reserve(h, &h->tc_Yt, &h->tc_Yt_bytes, lines * 4 * (size_t)g.Lty * sizeof(float))) return 1;
-  const size_t a_bytes = lines * (size_t)g.nchunk * 2 * tc::kATileBytes;
+  const size_t img_bytes = tc::a_image_bytes(lines, nchunk), a_bytes = img_bytes + lines * sizeof(int);
   const bool a_stale = h->tc_A_for != P.H || h->tc_A_P != P.Ppad || h->tc_A_B != P.B || h->tc_A_C != C || h->tc_A_bytes < a_bytes;
   if (a_stale) {
     h->tc_A_for = nullptr;
     if (!tc_reserve(h, &h->tc_A, &h->tc_A_bytes, a_bytes)) return 1;
   }
+  __half* A = static_cast<__half*>(h->tc_A);
+  int* eh = reinterpret_cast<int*>(static_cast<unsigned char*>(h->tc_A) + img_bytes);
   if (!h->tc_attr_set) {
-    CU_CHECK(h, cudaFuncSetAttribute(tc::k_tc_sweep, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::kSmemBytes));
+    CU_CHECK(h, cudaFuncSetAttribute(tc::k_tc_sweep, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::kSmemBytesF16));
     h->tc_attr_set = true;
   }
   cudaStream_t st = h->s_launch;
   int id = timing_begin(h, kKindCmac);
-  if (a_stale) {     // once per IR (and stage): H -> tf32 hi / lo Toeplitz tile images
-    tc::BuildAParams bp{P.H, P.h_cstride, P.B, P.Ppad, g.Q, g.nchunk, h->tc_A};
-    tc::k_tc_build_a<<<dim3(g.nchunk, P.B, C), 256, 0, st>>>(bp);
+  if (a_stale) {     // once per IR (and stage): H -> scaled FP16 hi / lo Toeplitz tile images and their exponents
+    tc::BuildAParams bp{P.H, P.h_cstride, P.B, P.Ppad, g.Q, nchunk, A, eh};
+    tc::k_tc_build_a<<<dim3(nchunk, P.B, C), 256, 0, st>>>(bp);
     h->tc_A_for = P.H; h->tc_A_P = P.Ppad; h->tc_A_B = P.B; h->tc_A_C = C;
     h->launches++;
   }
   tc::SplitXParams sp{P.X, P.x_cstride, P.xrow0 - g.Q, std::max<long long>(0, P.xrow0 - (P.Ppad - 1)), P.xrow0 + P.nblocks, P.B, g.rows, h->tc_Xt};
   tc::k_tc_split_x<<<dim3((unsigned)(g.rows * 2), P.B / 32, C), dim3(32, 8), 0, st>>>(sp);
-  tc::SweepParams wp{h->tc_A, h->tc_Xt, h->tc_Yt, (int)lines, g.ntile, g.nchunk, g.rows, g.Lty, h->tc_err_dev};
+  tc::SweepParams wp{A, eh, h->tc_Xt, h->tc_Yt, (int)lines, g.ntile, nchunk, g.rows, g.Lty, h->tc_err_dev};
   const int total = (int)lines * g.ntile;
-  tc::k_tc_sweep<<<std::min(total, h->n_sm), tc::kThreads, tc::kSmemBytes, st>>>(wp);
+  tc::k_tc_sweep<<<std::min(total, h->n_sm), tc::kThreads, tc::kSmemBytesF16, st>>>(wp);
   tc::MergeYParams mp{h->tc_Yt, g.Lty, P.B, P.nblocks, P.Y, P.y_cstride, P.y_rstride, P.yrow0};
   tc::k_tc_merge_y<<<dim3((P.nblocks + 31) / 32, P.B / 32, C), dim3(32, 8), 0, st>>>(mp);
   timing_end(h, id);
@@ -812,7 +816,7 @@ int launch_cmac(b200conv* h, const pc::CmacParams& P, int C) {
     else variant = (P.nblocks >= 64) ? 22 : 26;
   }
   h->last_variant = variant;
-  if (variant == 40) {                         // wgmma 3xTF32 block-Toeplitz sweep
+  if (variant == 40) {                         // wgmma 3xFP16 block-Toeplitz sweep
     if (!tc_eligible(h, P, C)) return fail(h, B200CONV_EINVAL, "tensor-core sweep: unsupported shape (needs B % 32 == 0, at most 961 partitions, no slot exchange)");
     const int rc = launch_cmac_tc(h, P, C);
     if (rc <= 0) return rc;

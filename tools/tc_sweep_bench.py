@@ -8,9 +8,11 @@ shape and batch of bench.py's headline.  Reported per library:
   * step time: CUDA events around one process_device call, L2 flushed before each, the libraries alternated round by
     round (`--rounds` rounds of `--steps` steps each), median and min - max;
   * per-kernel device time per step from torch.profiler (a separate pass after the timed one);
-  * k_tc_sweep's executed tf32 rate: tiles x K chunks x 24 MMAs of 2*128*64*8 flop (3xTF32 split x 2 time lines x 4
-    k-steps, counted as m64n64k8 products: the arithmetic is the same at any MMA shape) over its profiled time;
-  * max |y - y_first| / peak against the first library's output of the same step.
+  * k_tc_sweep's executed tensor rate: tiles x (Q/32 + 2) x 24 MMAs of 2*128*64*8 flop over its profiled time, and
+    that rate over the data sheet's dense FP16 rate (989 TFLOP/s, H100 SXM at 700 W).  The FP16 kernel executes
+    (Q/64 + 1) K chunks x 12 m64n128k16 MMAs (3xFP16 split x 4 k-steps) x 2 time lines: the same flop count;
+  * max |y - y_first| / peak against the first library's output of the same step (a build of the earlier tf32 form as
+    the first library shows how far the FP16 form moved the outputs).
 The card's name, power limit and SM clocks are read in the same run.  Needs a GPU; there is no CPU path."""
 from __future__ import annotations
 
@@ -31,6 +33,7 @@ from reevr_b200.convolver import Engine  # noqa: E402
 from reevr_b200.synth import synth_input, synth_ir  # noqa: E402
 
 C, SR, IR_S, BLOCK, T = 2, 48000, 10, 512, 112608
+FP16_DENSE_TFLOPS = 989.0               # H100 SXM data sheet, dense FP16 / BF16 with FP32 accumulate
 
 
 def card_info() -> dict:
@@ -144,6 +147,7 @@ def main() -> None:
         res["libs"][name] = {
             "step_ms_median": statistics.median(ts), "step_ms_min": min(ts), "step_ms_max": max(ts), "steps": len(ts),
             "k_tc_sweep_ms": sweep_ms, "k_tc_sweep_tflops": flop / (sweep_ms * 1e-3) / 1e12 if sweep_ms > 0 else None,
+            "k_tc_sweep_frac_of_fp16_dense": flop / (sweep_ms * 1e-3) / 1e12 / FP16_DENSE_TFLOPS if sweep_ms > 0 else None,
             "max_err_vs_" + first: parity[name],
             "kernels_ms_per_step": {k: round(v, 4) for k, v in kernels[name].items()},
         }
