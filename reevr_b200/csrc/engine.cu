@@ -43,9 +43,7 @@
 #include "kernels_fft512.cuh"
 #include "kernels_rt.cuh"
 #include "kernels_chain.cuh"
-#if !defined(PC_EMULATE)
 #include "kernels_tc.cuh"
-#endif
 
 namespace {
 
@@ -76,6 +74,9 @@ struct Stage {
   float2* H = nullptr;
   float2* X = nullptr;
   float2* Y[2] = {nullptr, nullptr};   // double buffer: the sweep of group i+1 may overlap reduce+IFFT of group i
+  // B = 512 groups on the tensor-core sweep: its bin-major complex result, read by the inverse FFT (paired with Y[b])
+  float2* tcY[2] = {nullptr, nullptr};
+  size_t tcY_bytes[2] = {0, 0};
   int ybuf = 0;
   cudaEvent_t ev_sweep[2] = {nullptr, nullptr};   // Y[b] rows written by the sweep
   cudaEvent_t ev_post[2] = {nullptr, nullptr};    // Y[b] no longer needed by reduce / inverse FFT
@@ -178,13 +179,14 @@ struct b200conv {
   bool opt_rt = std::getenv("B200CONV_NO_RT") == nullptr;
   bool opt_fft512 = std::getenv("B200CONV_NO_FFT512") == nullptr;
   bool opt_slice_tail = true;        // sliced calls: also transform the last P blocks of the call (full-state contract)
-  // tensor-core sweep (kernels_tc.cuh): Toeplitz tile images of one stage's H, per-bin time lines, partial planes
+  // tensor-core sweep (kernels_tc.cuh): Toeplitz tile images of one stage's H, per-bin time lines, the bin-major
+  // complex result of the groups that merge it into Y rows
   bool opt_tc = std::getenv("B200CONV_NO_TC") == nullptr;
   void* tc_A = nullptr;              // FP16 images, then the per-line scale exponents (kernels_tc.cuh a_image_bytes)
   const void* tc_A_for = nullptr;    // H the images were built from (+ its geometry)
   int tc_A_P = 0, tc_A_B = 0, tc_A_C = 0;
   float* tc_Xt = nullptr;
-  float* tc_Yt = nullptr;
+  float2* tc_Yt = nullptr;
   size_t tc_A_bytes = 0, tc_Xt_bytes = 0, tc_Yt_bytes = 0;
   int* tc_err = nullptr;             // mapped pinned word: a barrier wait of k_tc_sweep gave up
   int* tc_err_dev = nullptr;
@@ -266,7 +268,7 @@ int cuda_fail(b200conv* h, cudaError_t e, const char* what) {
 int fail(b200conv* h, int code, const std::string& msg) { h->err = msg; return code; }
 
 void free_stage(Stage& s) {
-  cudaFree(s.H); cudaFree(s.X); cudaFree(s.Y[0]); cudaFree(s.Y[1]); cudaFree(s.tw); cudaFree(s.tab512); cudaFree(s.inbuf); cudaFree(s.inbuf_alt); cudaFree(s.fut);
+  cudaFree(s.H); cudaFree(s.X); cudaFree(s.Y[0]); cudaFree(s.Y[1]); cudaFree(s.tcY[0]); cudaFree(s.tcY[1]); cudaFree(s.tw); cudaFree(s.tab512); cudaFree(s.inbuf); cudaFree(s.inbuf_alt); cudaFree(s.fut);
   for (int i = 0; i < 2; ++i) {
     if (s.ev_job[i]) cudaEventDestroy(s.ev_job[i]);
     if (s.ev_sweep[i]) cudaEventDestroy(s.ev_sweep[i]);
@@ -299,7 +301,7 @@ void free_all(b200conv* h) {
   }
   cudaFree(h->dch[0]); h->dch[0] = nullptr;
   cudaFree(h->tc_A); cudaFree(h->tc_Xt); cudaFree(h->tc_Yt);
-  h->tc_A = h->tc_Xt = h->tc_Yt = nullptr; h->tc_A_for = nullptr; h->tc_A_bytes = h->tc_Xt_bytes = h->tc_Yt_bytes = 0;
+  h->tc_A = h->tc_Xt = nullptr; h->tc_Yt = nullptr; h->tc_A_for = nullptr; h->tc_A_bytes = h->tc_Xt_bytes = h->tc_Yt_bytes = 0;
   if (h->tc_err) cudaFreeHost(h->tc_err);
   h->tc_err = h->tc_err_dev = nullptr; h->tc_alloc_failed = false;
   cudaFree(h->c_io); cudaFree(h->c_conv_in); cudaFree(h->c_filt); cudaFree(h->c_state); cudaFree(h->c_ring);
@@ -473,17 +475,25 @@ int launch_inv(b200conv* h, const pc::InvParams& P, int C, cudaStream_t st) {
                       (P.index0 & 1) == 0 && (P.dst_cstride & 1) == 0 && (reinterpret_cast<size_t>(P.dst) & 7) == 0;
     int id = timing_begin(h, kKindIfft, st);
 #if defined(PC_EMULATE)
+    if (P.yc) return fail(h, B200CONV_EINVAL, "bin-major input is not part of the CPU emulation");
     pc::emu_inv_fft512(P.nblocks, C, P, P.tab512, fast);
 #else
     const int gx = std::max(1, std::min((P.nblocks + 7) / 8, (3 * h->n_sm + C - 1) / C));
-    if (fast) pc::k_inv_fft512<true><<<dim3(gx, C, 1), dim3(32, 8, 1), kF512Smem, st>>>(P, P.tab512);
-    else pc::k_inv_fft512<false><<<dim3(gx, C, 1), dim3(32, 8, 1), kF512Smem, st>>>(P, P.tab512);
+    const dim3 grid(gx, C, 1), block(32, 8, 1);
+    if (P.yc) {
+      if (fast) pc::k_inv_fft512<true, true><<<grid, block, kF512Smem, st>>>(P, P.tab512);
+      else pc::k_inv_fft512<false, true><<<grid, block, kF512Smem, st>>>(P, P.tab512);
+    } else {
+      if (fast) pc::k_inv_fft512<true, false><<<grid, block, kF512Smem, st>>>(P, P.tab512);
+      else pc::k_inv_fft512<false, false><<<grid, block, kF512Smem, st>>>(P, P.tab512);
+    }
 #endif
     timing_end(h, id, st);
     h->launches++;
     CU_CHECK(h, cudaGetLastError());
     return 0;
   }
+  if (P.yc) return fail(h, B200CONV_EINVAL, "bin-major input needs the B = 512 inverse FFT");
   const FftGeom g = fft_geometry(P.M, P.nblocks, C);
   int id = timing_begin(h, kKindIfft, st);
 #if defined(PC_EMULATE)
@@ -744,10 +754,34 @@ bool tc_reserve(b200conv* h, T** buf, size_t* have, size_t need) {
 }
 #endif
 
-// returns 1 when the scratch could not be allocated (nothing launched), 0 on success, < 0 on error
-int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C) {
+// B = 512 launch groups on the tensor-core sweep (run_group): the sweep's bin-major complex result stays in Yc for the
+// inverse FFT; output 0 of the sweep is block -extra of the group (extra = 1: the sweep computes the overlap state)
+struct TcDirect {
+  float2* Yc;
+  int extra;
+};
+
+#if !defined(PC_EMULATE)
+// the scratch of a tensor-core sweep: time lines, Toeplitz images and the result lines (*yc); false: not enough memory
+bool tc_reserve_all(b200conv* h, const pc::CmacParams& P, int C, float2** yc, size_t* yc_bytes) {
+  namespace tc = pc::tc;
+  const tc::Geom g = tc::make_geom(P.Ppad, P.nblocks);
+  const size_t lines = (size_t)C * P.B;
+  if (!tc_reserve(h, &h->tc_Xt, &h->tc_Xt_bytes, lines * 2 * (size_t)g.Lt * sizeof(float))) return false;
+  if (!tc_reserve(h, yc, yc_bytes, lines * (size_t)tc::yc_stride(g) * sizeof(float2))) return false;
+  const size_t a_bytes = tc::a_image_bytes(lines, tc::nchunk_f16(g.Q)) + lines * sizeof(int);
+  if (h->tc_A_for != P.H || h->tc_A_P != P.Ppad || h->tc_A_B != P.B || h->tc_A_C != C || h->tc_A_bytes < a_bytes) {
+    h->tc_A_for = nullptr;
+    if (!tc_reserve(h, &h->tc_A, &h->tc_A_bytes, a_bytes)) return false;
+  }
+  return true;
+}
+#endif
+
+// the scratch is in place (tc_reserve_all); d != nullptr: the B = 512 direct form
+int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C, const TcDirect* d) {
 #if defined(PC_EMULATE)
-  (void)P; (void)C;
+  (void)P; (void)C; (void)d;
   return fail(h, B200CONV_EINVAL, "the tensor-core sweep is not part of the CPU emulation");
 #else
   namespace tc = pc::tc;
@@ -761,14 +795,8 @@ int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C) {
   if (*reinterpret_cast<volatile int*>(h->tc_err) != 0)
     return fail(h, B200CONV_ECUDA, "tensor-core sweep: a pipeline barrier timed out (code " + std::to_string(*h->tc_err) + ")");
   const int nchunk = tc::nchunk_f16(g.Q);
-  if (!tc_reserve(h, &h->tc_Xt, &h->tc_Xt_bytes, lines * 2 * (size_t)g.Lt * sizeof(float))) return 1;
-  if (!tc_reserve(h, &h->tc_Yt, &h->tc_Yt_bytes, lines * 4 * (size_t)g.Lty * sizeof(float))) return 1;
-  const size_t img_bytes = tc::a_image_bytes(lines, nchunk), a_bytes = img_bytes + lines * sizeof(int);
-  const bool a_stale = h->tc_A_for != P.H || h->tc_A_P != P.Ppad || h->tc_A_B != P.B || h->tc_A_C != C || h->tc_A_bytes < a_bytes;
-  if (a_stale) {
-    h->tc_A_for = nullptr;
-    if (!tc_reserve(h, &h->tc_A, &h->tc_A_bytes, a_bytes)) return 1;
-  }
+  const size_t img_bytes = tc::a_image_bytes(lines, nchunk);
+  const bool a_stale = h->tc_A_for != P.H || h->tc_A_P != P.Ppad || h->tc_A_B != P.B || h->tc_A_C != C;
   __half* A = static_cast<__half*>(h->tc_A);
   int* eh = reinterpret_cast<int*>(static_cast<unsigned char*>(h->tc_A) + img_bytes);
   if (!h->tc_attr_set) {
@@ -785,20 +813,26 @@ int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C) {
   }
   tc::SplitXParams sp{P.X, P.x_cstride, P.xrow0 - g.Q, std::max<long long>(0, P.xrow0 - (P.Ppad - 1)), P.xrow0 + P.nblocks, P.B, g.rows, h->tc_Xt};
   tc::k_tc_split_x<<<dim3((unsigned)(g.rows * 2), P.B / 32, C), dim3(32, 8), 0, st>>>(sp);
-  tc::SweepParams wp{A, eh, h->tc_Xt, h->tc_Yt, (int)lines, g.ntile, nchunk, g.rows, g.Lty, h->tc_err_dev};
+  float2* Yc = d ? d->Yc : h->tc_Yt;
+  tc::SweepParams wp{A, eh, h->tc_Xt, Yc, tc::yc_stride(g), (int)lines, g.ntile, nchunk, g.rows, P.B, h->tc_err_dev};
   const int total = (int)lines * g.ntile;
   tc::k_tc_sweep<<<std::min(total, h->n_sm), tc::kThreads, tc::kSmemBytesF16, st>>>(wp);
-  tc::MergeYParams mp{h->tc_Yt, g.Lty, P.B, P.nblocks, P.Y, P.y_cstride, P.y_rstride, P.yrow0};
-  tc::k_tc_merge_y<<<dim3((P.nblocks + 31) / 32, P.B / 32, C), dim3(32, 8), 0, st>>>(mp);
+  if (!d) {
+    tc::MergeYParams mp{Yc, tc::yc_stride(g), P.B, P.nblocks, P.Y, P.y_cstride, P.y_rstride, P.yrow0};
+    tc::k_tc_merge_y<<<dim3((P.nblocks + 31) / 32, P.B / 32, C), dim3(32, 8), 0, st>>>(mp);
+  }
   timing_end(h, id);
-  h->launches += 3;
+  h->launches += d ? 2 : 3;
   CU_CHECK(h, cudaGetLastError());
   return 0;
 #endif
 }
 
+// The sweep form of a launch (*variant).  A launch group decides it before its forward FFT: the tensor-core form
+// reserves its scratch here, so that when the memory is not there the FFMA sweep still finds the X rows it reads.
+// yc: where the tensor-core result lines go (the B = 512 direct form); nullptr: the handle's lines merged into Y rows.
 // P.Ppad enters as the number of real (unpadded) partition rows of this shard
-int launch_cmac(b200conv* h, const pc::CmacParams& P, int C) {
+int select_cmac(b200conv* h, const pc::CmacParams& P, int C, float2** yc, size_t* yc_bytes, int* variant_out) {
   int variant = h->cfg.cmac_variant;
   if (P.xg > 0) variant = (P.nblocks >= 64) ? 22 : 26;     // slot exchange: only the packed-FMA sweeps carry the exchange epilogue
   if (variant == 0) {
@@ -815,15 +849,25 @@ int launch_cmac(b200conv* h, const pc::CmacParams& P, int C) {
     else if (h->opt_tc && !h->tc_alloc_failed && P.nblocks >= kTcMinBlocks && tc_eligible(h, P, C)) variant = 40;
     else variant = (P.nblocks >= 64) ? 22 : 26;
   }
-  h->last_variant = variant;
   if (variant == 40) {                         // wgmma 3xFP16 block-Toeplitz sweep
     if (!tc_eligible(h, P, C)) return fail(h, B200CONV_EINVAL, "tensor-core sweep: unsupported shape (needs B % 32 == 0, at most 961 partitions, no slot exchange)");
-    const int rc = launch_cmac_tc(h, P, C);
-    if (rc <= 0) return rc;
-    if (h->cfg.cmac_variant == 40) return fail(h, B200CONV_ENOMEM, "tensor-core sweep: scratch allocation failed");
-    variant = (P.nblocks >= 64) ? 22 : 26;     // not enough device memory for the scratch: FFMA sweep
-    h->last_variant = variant;
+#if !defined(PC_EMULATE)
+    if (!tc_reserve_all(h, P, C, yc ? yc : &h->tc_Yt, yc ? yc_bytes : &h->tc_Yt_bytes)) {
+      if (h->cfg.cmac_variant == 40) return fail(h, B200CONV_ENOMEM, "tensor-core sweep: scratch allocation failed");
+      variant = (P.nblocks >= 64) ? 22 : 26;   // not enough device memory for the scratch: FFMA sweep
+    }
+#else
+    (void)yc; (void)yc_bytes;
+#endif
   }
+  h->last_variant = variant;
+  *variant_out = variant;
+  return 0;
+}
+
+// runs the sweep form select_cmac chose; td: the B = 512 direct form of a tensor-core launch group
+int launch_cmac_as(b200conv* h, const pc::CmacParams& P, int C, int variant, const TcDirect* td) {
+  if (variant == 40) return launch_cmac_tc(h, P, C, td);
   if (variant == 108) {                        // 6 stages x 2 CTAs/SM, skewed static slices (B200CONV_STREAM_SKEW percent, default 8)
     if (P.nblocks != 1 || P.B < 64) return fail(h, B200CONV_EINVAL, "TMA streaming sweep needs nblocks == 1 and B >= 64");
     static const float skew = [] { const char* e = std::getenv("B200CONV_STREAM_SKEW"); return e ? (float)std::atof(e) / 100.0f : 0.08f; }();
@@ -876,6 +920,12 @@ int launch_cmac(b200conv* h, const pc::CmacParams& P, int C) {
   h->launches++;
   CU_CHECK(h, cudaGetLastError());
   return 0;
+}
+
+int launch_cmac(b200conv* h, const pc::CmacParams& P, int C) {
+  int variant = 0;
+  if (int rc = select_cmac(h, P, C, nullptr, nullptr, &variant)) return rc;
+  return launch_cmac_as(h, P, C, variant, nullptr);
 }
 
 // the single-block sweep of a tail block whose partial spectrum goes to rank 0 through the slot exchange: the TMA
@@ -1657,8 +1707,27 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
     if (!direct) { if (int rc = copy_in(h, s.inbuf + s.fill, s.in_stride, in_dev, in_stride, n)) return rc; }
     const int yb = s.ybuf;
     float2* Yb = s.Y[yb];
+    // B = 512 groups on the tensor-core sweep (unsharded): the inverse FFT reads the sweep's bin-major result
+    // (tcY[yb]); the transpose into Y rows is left out
+    bool tc_direct = false;
+    TcDirect td{};
+    long long yc_stride = 0;
     if (nb > 0) {
       if (s.head + nb + kMaxTT > s.R) { if (int rc = compact_timeline(h, s)) return rc; }
+      // overlap state after a forward-FFT-only advance (time-slice sharding): Y row 0 must become
+      // sum_p H[p] X[head-1-p], the spectrum of the block in front of this group — its input spectra are in the
+      // timeline, so the sweep simply starts one block early and writes that block as row 0
+      const int extra = (si == 0 && h->yprev_stale) ? 1 : 0;
+      pc::CmacParams cp{};
+      cp.H = s.H; cp.h_cstride = (long long)s.Prows * B;
+      cp.X = s.X; cp.x_cstride = (long long)s.R * B; cp.xrow0 = s.head - s.p_begin - extra;
+      cp.Y = Yb; cp.y_cstride = B; cp.y_rstride = (long long)row; cp.yrow0 = 1 - extra;
+      cp.B = B; cp.Ppad = s.P; cp.nblocks = nb + extra;
+      const bool direct_ok = h->cfg.shard_count == 1 && use_fft512(h, B, nb, C, s.tab512);
+      int variant = 0;
+      if (int rc = select_cmac(h, cp, C, direct_ok ? &s.tcY[yb] : nullptr, &s.tcY_bytes[yb], &variant)) return rc;
+      tc_direct = direct_ok && variant == 40;
+
       pc::FwdParams fp{};
       fp.src = direct ? in_dev : s.inbuf;
       fp.src_cstride = direct ? (long long)in_stride : (long long)s.in_stride;
@@ -1666,24 +1735,19 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
       set_cmap(h, fp, direct);
       fp.dst = s.X; fp.dst_cstride = (long long)s.R * B; fp.dst_row0 = s.head;
       fp.tw = s.tw; fp.tab512 = s.tab512; fp.M = B; fp.nblocks = nb;
+      if (tc_direct) {
+        td.Yc = s.tcY[yb]; td.extra = extra;
+        yc_stride = pc::tc::yc_stride(pc::tc::make_geom(cp.Ppad, cp.nblocks));
+      }
       if (int rc = launch_fwd(h, fp, C)) return rc;
 
-      // Y[yb] rows >= 1 may still be read by the post work of two groups ago
+      // Y[yb] rows >= 1 (and tcY[yb]) may still be read by the post work of two groups ago
       if (overlap) CU_CHECK(h, cudaStreamWaitEvent(h->s_main, s.ev_post[yb], 0));
-      // overlap state after a forward-FFT-only advance (time-slice sharding): Y row 0 must become
-      // sum_p H[p] X[head-1-p], the spectrum of the block in front of this group — its input spectra are in the
-      // timeline, so the sweep simply starts one block early and writes that block as row 0
-      const int extra = (si == 0 && h->yprev_stale) ? 1 : 0;
       if (extra) {
         if (overlap) CU_CHECK(h, cudaStreamWaitEvent(h->s_main, s.ev_post[yb ^ 1], 0));   // row 0 was written on s_post
         h->yprev_stale = false;
       }
-      pc::CmacParams cp{};
-      cp.H = s.H; cp.h_cstride = (long long)s.Prows * B;
-      cp.X = s.X; cp.x_cstride = (long long)s.R * B; cp.xrow0 = s.head - s.p_begin - extra;
-      cp.Y = Yb; cp.y_cstride = B; cp.y_rstride = (long long)row; cp.yrow0 = 1 - extra;
-      cp.B = B; cp.Ppad = s.P; cp.nblocks = nb + extra;
-      if (int rc = launch_cmac(h, cp, C)) return rc;
+      if (int rc = launch_cmac_as(h, cp, C, variant, tc_direct ? &td : nullptr)) return rc;
       if (overlap) {
         CU_CHECK(h, cudaEventRecord(s.ev_sweep[yb], h->s_main));
         CU_CHECK(h, cudaStreamWaitEvent(ps, s.ev_sweep[yb], 0));
@@ -1698,6 +1762,10 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
         pc::InvParams ip{};
         ip.Y = Yb; ip.y_cstride = B; ip.y_rstride = (long long)row; ip.yrow0 = 1;
         ip.tw = s.tw; ip.tab512 = s.tab512; ip.M = B; ip.nblocks = nb; ip.scale = 1.0f / (float)B;
+        if (tc_direct) {   // block t at slot kYLead + extra + t; block -1 is the overlap state (Y row 0) unless swept
+          ip.yc = td.Yc; ip.yc_stride = yc_stride; ip.yc_slot0 = pc::tc::kYLead + td.extra;
+          ip.yc_prev_row = td.extra == 0;
+        }
         if (si == 0) {
           ip.dst = h->route_on ? h->dch[0] : out_dev;
           ip.dst_cstride = h->route_on ? (long long)h->Lmax : (long long)out_stride;
@@ -1724,8 +1792,12 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
     if (complete > 0) {
       // overlap state for the next group: last completed row -> row 0 of the buffer it will use
       const int nxt = overlap ? (yb ^ 1) : yb;
-      CU_CHECK(h, cudaMemcpyAsync(s.Y[nxt], Yb + (size_t)complete * row, row * sizeof(float2),
-                                  cudaMemcpyDeviceToDevice, ps));
+      if (tc_direct)     // block complete - 1 of every line
+        CU_CHECK(h, cudaMemcpy2DAsync(s.Y[nxt], sizeof(float2), td.Yc + pc::tc::kYLead + td.extra + (complete - 1),
+                                      (size_t)yc_stride * sizeof(float2), sizeof(float2), row, cudaMemcpyDeviceToDevice, ps));
+      else
+        CU_CHECK(h, cudaMemcpyAsync(s.Y[nxt], Yb + (size_t)complete * row, row * sizeof(float2),
+                                    cudaMemcpyDeviceToDevice, ps));
       if (overlap) CU_CHECK(h, cudaEventRecord(s.ev_post[yb], ps));
       s.ybuf = nxt;
       if (partial > 0) {
@@ -2094,8 +2166,10 @@ b200conv_t* b200conv_create(const b200conv_config* cfg) {
       attr_ok = attr_ok && rt_set_attr<16>() && rt_set_attr<32>() && rt_set_attr<64>() && rt_set_attr<128>() &&
                 rt_set_attr<256>() && rt_set_attr<512>() && rt_set_attr<1024>();
       attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_fwd_fft512, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
-      attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
-      attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
+      attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
+      attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
+      attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
+      attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
     });
     ok = attr_ok;
   }

@@ -601,6 +601,12 @@ struct InvParams {
   const float* add[3]; long long add_cstride[3]; long long add_mask[3];
   long long abs0;            // absolute stream position of sample 0 of block 0
   const float2* tab512;      // tables of the register-resident B = 512 kernels (kernels_fft512.cuh), else nullptr
+  // bin-major input (k_inv_fft512 only; the tensor-core sweep's result): block t of line c * M + k at
+  // yc[line * yc_stride + yc_slot0 + t], its predecessor one slot before.  yc_prev_row: block 0's predecessor is Y row
+  // yrow0 - 1 instead.  yc == nullptr: rows of Y
+  const float2* yc;
+  long long yc_stride, yc_slot0;
+  int yc_prev_row;
 };
 
 struct StreamParams {

@@ -233,21 +233,13 @@ PC_HD void f512_unsplit_pair(float2 a, float2 bm, float2 w, float2* zk, float2* 
   *zmk = make_float2(E.x + O.y, O.x - E.y);
 }
 
-// first inverse step: loads + merge + un-split + inverse DFT8 over q1 + twiddle -> exchange buffer (layout s2)
-PC_HD void f512_inv_p1(int lane, const float2* Yt, const float2* Yp, float2* S, const float2* tab) {
+// overlap-add merge of one bin k: W = Y[t] + (-1)^k Y[t - 1]
+PC_HD float2 f512_ola(float2 yt, float2 yp, float sg) { return make_float2(fmaf(yp.x, sg, yt.x), fmaf(yp.y, sg, yt.y)); }
+
+// first inverse step after the merge (A[q1] = W[la + 64 q1], B[q1] = W[lb + 64 q1]): un-split + inverse DFT8 over q1
+// + twiddle -> exchange buffer (layout s2)
+PC_HD void f512_inv_p1_core(int lane, float2* A, float2* B, float2* S, const float2* tab) {
   const int la = f512_la(lane), lb = f512_lb(lane);
-  float2 A[8], B[8], PA[8], PB[8];
-#pragma unroll
-  for (int q1 = 0; q1 < 8; ++q1) {       // all 32 loads first
-    A[q1] = PC_LD(Yt + la + 64 * q1); B[q1] = PC_LD(Yt + lb + 64 * q1);
-    PA[q1] = PC_LD(Yp + la + 64 * q1); PB[q1] = PC_LD(Yp + lb + 64 * q1);
-  }
-  const float sg = (lane & 1) ? -1.0f : 1.0f;          // (-1)^k: k has the parity of the lane for both residues
-#pragma unroll
-  for (int q1 = 0; q1 < 8; ++q1) {
-    A[q1] = make_float2(fmaf(PA[q1].x, sg, A[q1].x), fmaf(PA[q1].y, sg, A[q1].y));
-    B[q1] = make_float2(fmaf(PB[q1].x, sg, B[q1].x), fmaf(PB[q1].y, sg, B[q1].y));
-  }
   float2 ZA[8], ZB[8];
   if (lane != 0) {
 #pragma unroll
@@ -271,6 +263,24 @@ PC_HD void f512_inv_p1(int lane, const float2* Yt, const float2* Yp, float2* S, 
     S[f512_s2(la & 7, la >> 3, n0)] = da;
     S[f512_s2(lb & 7, lb >> 3, n0)] = db;
   }
+}
+
+// first inverse step from rows: loads of Y[t] (Yt) and Y[t - 1] (Yp) + merge + the rest of the step
+PC_HD void f512_inv_p1(int lane, const float2* Yt, const float2* Yp, float2* S, const float2* tab) {
+  const int la = f512_la(lane), lb = f512_lb(lane);
+  float2 A[8], B[8], PA[8], PB[8];
+#pragma unroll
+  for (int q1 = 0; q1 < 8; ++q1) {       // all 32 loads first
+    A[q1] = PC_LD(Yt + la + 64 * q1); B[q1] = PC_LD(Yt + lb + 64 * q1);
+    PA[q1] = PC_LD(Yp + la + 64 * q1); PB[q1] = PC_LD(Yp + lb + 64 * q1);
+  }
+  const float sg = (lane & 1) ? -1.0f : 1.0f;          // (-1)^k: k has the parity of the lane for both residues
+#pragma unroll
+  for (int q1 = 0; q1 < 8; ++q1) {
+    A[q1] = f512_ola(A[q1], PA[q1], sg);
+    B[q1] = f512_ola(B[q1], PB[q1], sg);
+  }
+  f512_inv_p1_core(lane, A, B, S, tab);
 }
 
 // last inverse step: inverse DFT8 over k2 for the two columns; only n2 < 4 (the first B of the 2B output samples)
@@ -339,7 +349,8 @@ __global__ void __launch_bounds__(256, 4) k_fwd_fft512(FwdParams P, const float2
   }
 }
 
-template <bool FAST>
+// YC: bin-major input (P.yc), 8 consecutive blocks per CTA
+template <bool FAST, bool YC>
 __global__ void __launch_bounds__(256, 3) k_inv_fft512(InvParams P, const float2* __restrict__ tab512) {
   extern __shared__ float2 pc_smem512[];
   float2* tab = pc_smem512;
@@ -357,19 +368,78 @@ __global__ void __launch_bounds__(256, 3) k_inv_fft512(InvParams P, const float2
     o.add[a] = a < P.n_add ? P.add[a] + (long long)c * P.add_cstride[a] : nullptr;
     o.add_mask[a] = P.add_mask[a];
   }
-  for (int blk = blockIdx.x * 8 + threadIdx.y; blk < P.nblocks; blk += gridDim.x * 8) {
-    o.index0 = P.index0 + (long long)blk * kF512_M;
-    o.abs0 = P.abs0 + (long long)blk * kF512_M;
-    const float2* Yt = P.Y + (long long)c * P.y_cstride + (P.yrow0 + blk) * P.y_rstride;
-    f512_inv_p1(lane, Yt, Yt - P.y_rstride, S, tab);
-    __syncwarp();
-    float2 A[8], B[8];
-    f512_mid_load<true>(lane, S, tab, A, B);
-    __syncwarp();
-    f512_mid_store<true>(lane, S, A, B);
-    __syncwarp();
-    f512_inv_p3<FAST>(lane, S, P.scale, o);
-    __syncwarp();
+  if (YC) {
+    // bin-major input: the CTA takes 8 consecutive blocks t0 ... t0 + 7, reads per bin the 9 spectra t0 - 1 ... t0 + 7
+    // of its line, and leaves the merged W[t] = Y[t] + (-1)^k Y[t - 1] in the exchange buffer of the warp of block t
+    float2* S0 = pc_smem512 + kF512_TabLen;
+    const int ngroups = (P.nblocks + 7) / 8;
+    for (int g = blockIdx.x; g < ngroups; g += gridDim.x) {
+      const int t0 = 8 * g;
+      const bool full = t0 + 8 <= P.nblocks;
+      __syncthreads();                                              // the previous group's reads of the buffers are done
+      for (int k = tid; k < kF512_M; k += 256) {
+        const float2* line = P.yc + ((long long)c * kF512_M + k) * P.yc_stride;
+        const long long s = P.yc_slot0 + t0 - 1;                    // slot of Y[t0 - 1]
+        float2 v[9];
+        if (full && (s & 1) == 0) {                                 // v[0 .. 7] in four aligned float4
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            const float4 f = __ldg(reinterpret_cast<const float4*>(line + s) + u);
+            v[2 * u] = make_float2(f.x, f.y); v[2 * u + 1] = make_float2(f.z, f.w);
+          }
+          v[8] = __ldg(line + s + 8);
+        } else if (full) {                                          // v[1 .. 8] in four aligned float4
+          v[0] = __ldg(line + s);
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            const float4 f = __ldg(reinterpret_cast<const float4*>(line + s + 1) + u);
+            v[2 * u + 1] = make_float2(f.x, f.y); v[2 * u + 2] = make_float2(f.z, f.w);
+          }
+        } else {
+#pragma unroll
+          for (int j = 0; j < 9; ++j) v[j] = t0 - 1 + j < P.nblocks ? __ldg(line + s + j) : make_float2(0.0f, 0.0f);
+        }
+        if (t0 == 0 && P.yc_prev_row) v[0] = P.Y[(long long)c * P.y_cstride + (P.yrow0 - 1) * P.y_rstride + k];
+        const float sg = (k & 1) ? -1.0f : 1.0f;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) S0[w * kF512_Xch + k] = f512_ola(v[w + 1], v[w], sg);
+      }
+      __syncthreads();
+      const int blk = t0 + threadIdx.y;
+      if (blk >= P.nblocks) continue;
+      o.index0 = P.index0 + (long long)blk * kF512_M;
+      o.abs0 = P.abs0 + (long long)blk * kF512_M;
+      {
+        const int la = f512_la(lane), lb = f512_lb(lane);
+        float2 A[8], B[8];
+#pragma unroll
+        for (int q1 = 0; q1 < 8; ++q1) { A[q1] = S[la + 64 * q1]; B[q1] = S[lb + 64 * q1]; }
+        __syncwarp();
+        f512_inv_p1_core(lane, A, B, S, tab);
+      }
+      __syncwarp();
+      float2 A[8], B[8];
+      f512_mid_load<true>(lane, S, tab, A, B);
+      __syncwarp();
+      f512_mid_store<true>(lane, S, A, B);
+      __syncwarp();
+      f512_inv_p3<FAST>(lane, S, P.scale, o);
+    }
+  } else {
+    for (int blk = blockIdx.x * 8 + threadIdx.y; blk < P.nblocks; blk += gridDim.x * 8) {
+      o.index0 = P.index0 + (long long)blk * kF512_M;
+      o.abs0 = P.abs0 + (long long)blk * kF512_M;
+      const float2* Yt = P.Y + (long long)c * P.y_cstride + (P.yrow0 + blk) * P.y_rstride;
+      f512_inv_p1(lane, Yt, Yt - P.y_rstride, S, tab);
+      __syncwarp();
+      float2 A[8], B[8];
+      f512_mid_load<true>(lane, S, tab, A, B);
+      __syncwarp();
+      f512_mid_store<true>(lane, S, A, B);
+      __syncwarp();
+      f512_inv_p3<FAST>(lane, S, P.scale, o);
+      __syncwarp();
+    }
   }
 }
 #else

@@ -37,10 +37,16 @@
 //
 // Kernels: k_tc_build_a (H -> FP16 hi/lo Toeplitz tile images and eh, once per IR), k_tc_split_x (timeline rows ->
 // per-bin FP32 time lines), k_tc_sweep (producer warpgroup: image ring + strip conversion / two MMA warpgroups
-// accumulating in registers), k_tc_merge_y (partial planes -> Y rows, combines the complex product).
+// accumulating in registers; the epilogue combines the complex product into bin-major float2 lines), k_tc_merge_y
+// (bin-major lines -> Y rows, for the groups whose inverse FFT reads rows).
 #pragma once
 
+#if defined(PC_EMULATE)                             // tests/emu: only the host-side geometry and layout functions
+#define PC_TC_HD inline
+#else
 #include <cuda_runtime.h>
+#define PC_TC_HD inline __host__ __device__
+#endif
 #include <cstdint>
 #if defined(__CUDACC__)
 #include <cuda_fp16.h>
@@ -70,7 +76,7 @@ struct Geom {
   long long Lt, Lty;
 };
 
-inline __host__ __device__ Geom make_geom(int P, int nb) {
+PC_TC_HD Geom make_geom(int P, int nb) {
   Geom g;
   g.P = P;
   g.Q = ((P > 1 ? P - 1 : 0) + 63) / 64 * 64;
@@ -83,13 +89,13 @@ inline __host__ __device__ Geom make_geom(int P, int nb) {
   g.Lty = (long long)g.ntile * kN * 64;
   return g;
 }
-inline __host__ __device__ bool geom_ok(const Geom& g, int B) { return g.nchunk <= kMaxChunks && B % 32 == 0 && g.nb > 0; }
+PC_TC_HD bool geom_ok(const Geom& g, int B) { return g.nchunk <= kMaxChunks && B % 32 == 0 && g.nb > 0; }
 
 // byte offset of element (row r, float e < 32) in a SWIZZLE_128B K-major image with a 1024-byte aligned base
-inline __host__ __device__ uint32_t sw128(uint32_t r, uint32_t e) { return r * 128u + ((((e >> 2) ^ (r & 7u)) & 7u) << 4) + (e & 3u) * 4u; }
+PC_TC_HD uint32_t sw128(uint32_t r, uint32_t e) { return r * 128u + ((((e >> 2) ^ (r & 7u)) & 7u) << 4) + (e & 3u) * 4u; }
 
 // tf32 time-line layout: [line][re_hi, re_lo, im_hi, im_lo][e][row R][32 floats], pre-swizzled
-inline __host__ __device__ size_t xt_index(long long line, int pl, int e, long long R, int jj, int rows) {
+PC_TC_HD size_t xt_index(long long line, int pl, int e, long long R, int jj, int rows) {
   return ((((size_t)line * 4 + pl) * 2 + e) * (size_t)rows + (size_t)R) * 32 + (size_t)(((((jj >> 2) ^ (int)(R & 7)) & 7) << 2) | (jj & 3));
 }
 
@@ -102,23 +108,28 @@ constexpr int kStripThreads = 96;                   // producer warps 9-11 conve
 // K chunks accumulated by the tensor core before the FP32 register add: 2 x 64 = the same K per chain as 4 x 32 tf32
 constexpr int kFlushF16 = 2;
 
-inline __host__ __device__ int nchunk_f16(int Q) { return Q / kChunkK + 1; }
+PC_TC_HD int nchunk_f16(int Q) { return Q / kChunkK + 1; }
 
 // byte offset of element (row r, half e < 64) in a SWIZZLE_128B K-major image with a 1024-byte aligned base
-inline __host__ __device__ uint32_t sw128_h(uint32_t r, uint32_t e) { return r * 128u + ((((e >> 3) ^ (r & 7u)) & 7u) << 4) + (e & 7u) * 2u; }
+PC_TC_HD uint32_t sw128_h(uint32_t r, uint32_t e) { return r * 128u + ((((e >> 3) ^ (r & 7u)) & 7u) << 4) + (e & 7u) * 2u; }
 
 // FP32 time lines: [line][re, im][rows * 64 samples]; sample tau sits in row tau / 64, so the 80 rows of tile nt's
 // strip are the contiguous samples 64 * 64 nt ... + 80 * 64
-inline __host__ __device__ size_t xf_index(long long line, int comp, long long tau, int rows) {
+PC_TC_HD size_t xf_index(long long line, int comp, long long tau, int rows) {
   return ((size_t)line * 2 + comp) * (size_t)rows * 64 + (size_t)tau;
 }
 
+// complex result: [line][ystride] float2, sweep output tau at slot kYLead + tau.  The lead slots in front of output 0
+// hold the block before it where the inverse FFT wants it there (its overlap-add reads every block's predecessor)
+constexpr int kYLead = 8;
+PC_TC_HD long long yc_stride(const Geom& g) { return g.Lty + 2 * kYLead; }
+
 // Toeplitz images: [line][chunk][hi, lo][128 rows x 64 halves], then eh of every line (int)
-inline __host__ __device__ size_t a_image_bytes(size_t lines, int nchunk) { return lines * (size_t)nchunk * 2 * kATileBytes; }
+PC_TC_HD size_t a_image_bytes(size_t lines, int nchunk) { return lines * (size_t)nchunk * 2 * kATileBytes; }
 
 // power-of-two exponent that puts a window's largest magnitude into [2^14, 2^15).  m = bit pattern of that magnitude
 // (sign cleared).  Zero and non-finite windows use 0: zeros stay exact zeros, NaN / Inf propagate unscaled.
-inline __host__ __device__ int scale_exp(uint32_t m) {
+PC_TC_HD int scale_exp(uint32_t m) {
   if (m == 0u || m >= 0x7f800000u) return 0;
   int E = (int)(m >> 23);                           // biased exponent: m in [2^(E-127), 2^(E-126))
   if (E == 0) {                                     // subnormal: the exponent of its leading bit
@@ -208,10 +219,10 @@ __global__ void __launch_bounds__(256) k_tc_split_x(SplitXParams p) {
   }
 }
 
-// ---- partial planes -> Y rows ----------------------------------------------------------------------------------
+// ---- bin-major complex lines -> Y rows -------------------------------------------------------------------------
 struct MergeYParams {
-  const float* Yt;          // [C*B lines][D part0, D part1, D2 part0, D2 part1][Lty]
-  long long Lty;
+  const float2* Yc;         // [C*B lines][ystride], output t at slot kYLead + t
+  long long ystride;
   int B, nb;
   float2* Y;
   long long y_cstride, y_rstride, yrow0;
@@ -225,13 +236,7 @@ __global__ void __launch_bounds__(256) k_tc_merge_y(MergeYParams p) {
   const int k0 = blockIdx.y * 32, ch = blockIdx.z;
   for (int kk = ty; kk < 32; kk += 8) {
     const long long line = (long long)ch * p.B + k0 + kk;
-    const float* src = p.Yt + line * 4 * p.Lty + t0 + tx;
-    float2 y = make_float2(0.0f, 0.0f);
-    if (t0 + tx < p.nb) {
-      const float d0 = src[0], d1 = src[p.Lty], e0 = src[2 * p.Lty], e1 = src[3 * p.Lty];
-      y = (k0 + kk == 0) ? make_float2(d0, e1) : make_float2(d0 - e1, d1 + e0);
-    }
-    tile[tx][kk] = y;
+    tile[tx][kk] = t0 + tx < p.nb ? p.Yc[line * p.ystride + kYLead + t0 + tx] : make_float2(0.0f, 0.0f);
   }
   __syncthreads();
   for (int r = ty; r < 32; r += 8) {
@@ -245,10 +250,10 @@ struct SweepParams {
   const __half* A;
   const int* eh;
   const float* Xt;
-  float* Yt;
-  int lines, ntile, nchunk, rows;
-  long long Lty;
-  int* err;                 // (mapped host word) set non-zero when a barrier wait gave up — a bug, not a data condition
+  float2* Yc;               // [lines][ystride] complex result, bin-major (kYLead)
+  long long ystride;
+  int lines, ntile, nchunk, rows, B;
+  int* err;                // (mapped host word) set non-zero when a barrier wait gave up — a bug, not a data condition
 };
 
 __device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
@@ -322,6 +327,61 @@ __device__ __forceinline__ void split_pair(float a, float b, uint32_t& hi, uint3
   const __half2 l = __floats2half2_rn(a - f.x, b - f.y);
   hi = *reinterpret_cast<const uint32_t*>(&h);
   lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+
+__device__ __forceinline__ void bar_sync_n(uint32_t id, uint32_t count) { asm volatile("bar.sync %0, %1;" :: "r"(id), "r"(count) : "memory"); }
+
+// Epilogue of MMA warpgroup CP (0: D = x_re [Hr ; Hi], 1: D2 = x_im [Hr ; Hi]) for one tile, acc scaled:
+//   y.re = D[i] - D2[64 + i],  y.im = D[64 + i] + D2[i]     (entry 0 = DC / Nyquist: y = (D[i], D2[64 + i]))
+// Warpgroup CP stores the output steps i in [32 CP, 32 CP + 32): fragment registers 4 j + r with j in KEEP = {4 CP ..
+// 4 CP + 3} (rows m = i) and 8 + KEEP (rows m = 64 + i).  It hands its other registers (j in GIVE and 8 + GIVE) to the
+// partner through `xch` (this tile's strip buffer; per warpgroup [32 registers][128 threads] floats over its own hi / lo
+// strips, which it stopped reading at its wg_wait<0>) and takes the partner's registers of its own positions into them.
+// The leader releases the buffer (`strip_empty`) once its warpgroup has read the partner's half.  The FP32 operations are one
+// __fsub_rn / __fadd_rn per component on the same operands as everywhere else this product is combined.
+template <int CP>
+__device__ __forceinline__ void tc_store_complex(float (&acc)[64], float* xch, unsigned long long* strip_empty, bool leader,
+                                                 bool dc, float2* dst, int wq, int lane, int t128) {
+  constexpr int KEEP = 4 * CP, GIVE = 4 - KEEP;
+  constexpr int kHalf = 2 * kStripBytes / 4;          // a warpgroup's own hi / lo strips: the partner may still read the other's
+  float* mine = xch + CP * kHalf;
+  const float* theirs = xch + (1 - CP) * kHalf;
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      mine[(q * 4 + r) * 128 + t128] = acc[4 * (GIVE + q) + r];
+      mine[((4 + q) * 4 + r) * 128 + t128] = acc[4 * (8 + GIVE + q) + r];
+    }
+  bar_sync_n(2, 256);
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      acc[4 * (GIVE + q) + r] = theirs[(q * 4 + r) * 128 + t128];
+      acc[4 * (8 + GIVE + q) + r] = theirs[((4 + q) * 4 + r) * 128 + t128];
+    }
+  bar_sync_n(3 + CP, 128);
+  if (leader) mbar_arrive1(strip_empty);
+  // register 4 j + r of lane l in warp wq: segment 16 wq + l / 4 + 8 (r / 2), row m = 8 j + 2 (l % 4) + (r % 2)
+  const int n0 = 16 * wq + (lane >> 2), i0 = 2 * (lane & 3);
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float y[4];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int r = 2 * h + e;
+        const float own_lo = acc[4 * (KEEP + q) + r], own_hi = acc[4 * (8 + KEEP + q) + r];
+        const float oth_lo = acc[4 * (GIVE + q) + r], oth_hi = acc[4 * (8 + GIVE + q) + r];
+        const float d0 = CP ? oth_lo : own_lo, d1 = CP ? oth_hi : own_hi;     // D[i], D[64 + i]
+        const float e0 = CP ? own_lo : oth_lo, e1 = CP ? own_hi : oth_hi;     // D2[i], D2[64 + i]
+        y[2 * e] = dc ? d0 : __fsub_rn(d0, e1);
+        y[2 * e + 1] = dc ? e1 : __fadd_rn(d1, e0);
+      }
+      *reinterpret_cast<float4*>(dst + (size_t)(n0 + 8 * h) * 64 + 8 * (KEEP + q) + i0) = make_float4(y[0], y[1], y[2], y[3]);
+    }
 }
 
 // grid: any (persistent, tiles walked round-robin); block 384 = MMA warpgroups 0 and 1 (warps 0-7), producer
@@ -506,10 +566,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_tc_sweep(SweepParams P) {
     wg_wait<0>();                                         // the last chain is complete: fold it, hand back the strips
     fence_operands(d0);
     fence_operands(d1);
-    if (leader) {
-      mbar_arrive1(&bar_a_empty[pending]);
-      mbar_arrive1(&bar_strip_empty[n & 1]);
-    }
+    if (leader) mbar_arrive1(&bar_a_empty[pending]);
     pending = -1;
     if ((P.nchunk + kFlushF16 - 1) / kFlushF16 & 1) {     // an odd number of chains ends in d0
 #pragma unroll
@@ -528,21 +585,11 @@ __global__ void __launch_bounds__(kThreads, 1) k_tc_sweep(SweepParams P) {
 #pragma unroll
       for (int j = 0; j < 64; ++j) acc[j] = ldexpf(acc[j], -e);
     }
-    // accumulator fragment of m64n128: register 4 j + r of lane l in warp wq holds segment 16 wq + l / 4 + 8 (r / 2) and
-    // Toeplitz row m = 8 j + 2 (l % 4) + (r % 2), i.e. output step m % 64 of plane comp * 2 + m / 64; registers 4 j + r
-    // and 4 j + r + 1 (r even) are consecutive steps
-    const int n0 = 16 * wq + (lane >> 2), i0 = 2 * (lane & 3);
-#pragma unroll
-    for (int part = 0; part < 2; ++part) {
-      float* dst = P.Yt + ((size_t)line * 4 + comp * 2 + part) * P.Lty + (size_t)nt * kN * 64;
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = 4 * (8 * part + j) + 2 * h;
-          *reinterpret_cast<float2*>(dst + (size_t)(n0 + 8 * h) * 64 + 8 * j + i0) = make_float2(acc[r], acc[r + 1]);
-        }
-    }
+    float* xch = reinterpret_cast<float*>(strips + (n & 1) * 4 * kStripBytes);
+    float2* dst = P.Yc + (size_t)line * P.ystride + kYLead + (size_t)nt * kN * 64;
+    const bool dc = line % P.B == 0;
+    if (comp == 0) tc_store_complex<0>(acc, xch, &bar_strip_empty[n & 1], leader, dc, dst, wq, lane, tid & 127);
+    else tc_store_complex<1>(acc, xch, &bar_strip_empty[n & 1], leader, dc, dst, wq, lane, tid & 127);
   }
 }
 
