@@ -431,6 +431,8 @@ bool stream_set_smem_attr() {
 // would pay the per-CTA table staging for nothing
 constexpr int kF512MinTransforms = 32;
 constexpr size_t kF512Smem = (size_t)(pc::kF512_TabLen + 8 * pc::kF512_Xch) * sizeof(float2);
+// k_fwd_fft512_lines: + the [re / im][512][16] time-line tile (2 CTAs per SM)
+constexpr size_t kF512LinesSmem = kF512Smem + (size_t)2 * pc::kF512_M * pc::kF512_LineR * sizeof(float);
 
 bool use_fft512(const b200conv* h, int M, int nblocks, int C, const float2* tab) {
   return h->opt_fft512 && M == pc::kF512_M && tab != nullptr && (long long)nblocks * C >= kF512MinTransforms;
@@ -440,10 +442,18 @@ int launch_fwd(b200conv* h, const pc::FwdParams& P, int C) {
   if (use_fft512(h, P.M, P.nblocks, C, P.tab512)) {
     int id = timing_begin(h, kKindFft);
 #if defined(PC_EMULATE)
+    if (P.lines) return fail(h, B200CONV_EINVAL, "time-line output is not part of the CPU emulation");
     pc::emu_fwd_fft512(P.nblocks, C, P, P.tab512);
 #else
-    const int gx = std::max(1, std::min((P.nblocks + 7) / 8, (4 * h->n_sm + C - 1) / C));
-    pc::k_fwd_fft512<<<dim3(gx, C, 1), dim3(32, 8, 1), kF512Smem, h->s_launch>>>(P, P.tab512);
+    if (P.lines) {
+      const long long R = pc::kF512_LineR;
+      const int tiles = (int)((P.line_tau0 + P.nblocks - 1) / R - P.line_tau0 / R + 1);
+      const int gx = std::max(1, std::min(tiles, (2 * h->n_sm + C - 1) / C));
+      pc::k_fwd_fft512_lines<<<dim3(gx, C, 1), dim3(32, 8, 1), kF512LinesSmem, h->s_launch>>>(P, P.tab512);
+    } else {
+      const int gx = std::max(1, std::min((P.nblocks + 7) / 8, (4 * h->n_sm + C - 1) / C));
+      pc::k_fwd_fft512<<<dim3(gx, C, 1), dim3(32, 8, 1), kF512Smem, h->s_launch>>>(P, P.tab512);
+    }
 #endif
     timing_end(h, id);
     h->launches++;
@@ -811,8 +821,13 @@ int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C, const TcDirect* 
     h->tc_A_for = P.H; h->tc_A_P = P.Ppad; h->tc_A_B = P.B; h->tc_A_C = C;
     h->launches++;
   }
-  tc::SplitXParams sp{P.X, P.x_cstride, P.xrow0 - g.Q, std::max<long long>(0, P.xrow0 - (P.Ppad - 1)), P.xrow0 + P.nblocks, P.B, g.rows, h->tc_Xt};
-  tc::k_tc_split_x<<<dim3((unsigned)(g.rows * 2), P.B / 32, C), dim3(32, 8), 0, st>>>(sp);
+  // the direct form's forward FFT wrote the group's own blocks (tau = Q + extra ... Q + nblocks - 1) into the time
+  // lines: the split only fills the history in front of them and zeroes the tail behind them
+  tc::SplitXParams sp{P.X, P.x_cstride, P.xrow0 - g.Q, std::max<long long>(0, P.xrow0 - (P.Ppad - 1)), P.xrow0 + P.nblocks, P.B, g.rows, h->tc_Xt,
+                      d ? g.Q + d->extra : g.Lt, d ? g.Q + P.nblocks : g.Lt, 0, 0};
+  tc::split_x_chunks(g.rows, sp.skip_lo, sp.skip_hi, &sp.nchunk_lo, &sp.chunk_hi);
+  const int split_chunks = sp.nchunk_lo + g.rows * 2 - sp.chunk_hi;
+  tc::k_tc_split_x<<<dim3((unsigned)split_chunks, P.B / 32, C), dim3(32, 8), 0, st>>>(sp);
   float2* Yc = d ? d->Yc : h->tc_Yt;
   tc::SweepParams wp{A, eh, h->tc_Xt, Yc, tc::yc_stride(g), (int)lines, g.ntile, nchunk, g.rows, P.B, h->tc_err_dev};
   const int total = (int)lines * g.ntile;
@@ -1737,7 +1752,15 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
       fp.tw = s.tw; fp.tab512 = s.tab512; fp.M = B; fp.nblocks = nb;
       if (tc_direct) {
         td.Yc = s.tcY[yb]; td.extra = extra;
-        yc_stride = pc::tc::yc_stride(pc::tc::make_geom(cp.Ppad, cp.nblocks));
+        const pc::tc::Geom tg = pc::tc::make_geom(cp.Ppad, cp.nblocks);
+        yc_stride = pc::tc::yc_stride(tg);
+        // the spectra go straight into the sweep's time lines (block b at tau = Q + extra + b).  X rows are still what
+        // everything after this group reads the history from: the next group's split, real-time calls and the
+        // streaming sweeps, FFMA groups, a time-slice rank's early block (its sweep starts one row back) and
+        // compact_timeline.  None of them reads further back than s.hist rows behind the head (compact_timeline
+        // keeps exactly those), so only the blocks from complete - s.hist on write their rows
+        fp.lines = h->tc_Xt; fp.line_tau0 = tg.Q + extra; fp.line_rows = tg.rows;
+        fp.xrow_from = std::max(0, complete - s.hist);
       }
       if (int rc = launch_fwd(h, fp, C)) return rc;
 
@@ -2168,6 +2191,7 @@ b200conv_t* b200conv_create(const b200conv_config* cfg) {
       attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_fwd_fft512, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
       attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
       attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
+      attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_fwd_fft512_lines, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512LinesSmem) == cudaSuccess;
       attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
       attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
     });

@@ -540,6 +540,13 @@ struct FwdParams {
   int use_cmap;              // routing: channel c reads source channel cmap[c] (StereoConvolver: LL,RR,LR,RL <- L,R,L,R)
   int cmap[8];
   const float2* tab512;      // tables of the register-resident B = 512 kernels (kernels_fft512.cuh), else nullptr
+  // time-line output (k_fwd_fft512_lines, B = 512 groups on the tensor-core sweep): block b of channel c is sample
+  // line_tau0 + b of the FP32 time lines of lines c * M ... c * M + M - 1 (tc::xf_index, line_rows rows of 64 samples);
+  // its X row is written only for b >= xrow_from.  lines == nullptr: X rows only
+  float* lines;
+  long long line_tau0;
+  int line_rows;
+  int xrow_from;
 };
 
 struct CmacParams {

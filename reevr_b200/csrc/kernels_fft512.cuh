@@ -32,6 +32,7 @@
 #pragma once
 
 #include "kernels.cuh"
+#include "kernels_tc.cuh"
 
 namespace pc {
 
@@ -191,8 +192,8 @@ PC_HD void f512_split_pair(float2 a, float2 bm, float2 w, float2* xk, float2* xm
   *xmk = make_float2(t.x, -t.y);
 }
 
-// step 3: DFT8 over n0 for both residues, split, packed spectrum row to global memory
-PC_HD void f512_fwd_p3(int lane, const float2* S, const float2* tab, float2* X) {
+// step 3: DFT8 over n0 for both residues and split: XA[q1] = X[la + 64 q1], XB[q1] = X[lb + 64 q1] of the packed spectrum
+PC_HD void f512_fwd_p3_core(int lane, const float2* S, const float2* tab, float2* XA, float2* XB) {
   const int la = f512_la(lane), lb = f512_lb(lane);
   float2 A[8], B[8];
 #pragma unroll
@@ -202,7 +203,6 @@ PC_HD void f512_fwd_p3(int lane, const float2* S, const float2* tab, float2* X) 
   }
   f512_dft8<false>(A);      // A[q1] = Z[la + 64 q1]
   f512_dft8<false>(B);      // B[q1] = Z[lb + 64 q1]
-  float2 XA[8], XB[8];
   if (lane != 0) {          // mirror of la + 64 q1 is lb + 64 (7 - q1)
 #pragma unroll
     for (int q1 = 0; q1 < 8; ++q1)
@@ -215,12 +215,31 @@ PC_HD void f512_fwd_p3(int lane, const float2* S, const float2* tab, float2* X) 
 #pragma unroll
     for (int q1 = 0; q1 < 4; ++q1) f512_split_pair(B[q1], B[7 - q1], tab[kF512_TS + 32 + 64 * q1], &XB[q1], &XB[7 - q1]);
   }
+}
+
+// packed spectrum row to global memory
+PC_HD void f512_fwd_store(int lane, const float2* XA, const float2* XB, float2* X) {
+  const int la = f512_la(lane), lb = f512_lb(lane);
 #pragma unroll
   for (int q1 = 0; q1 < 8; ++q1) {
     X[la + 64 * q1] = XA[q1];
     X[lb + 64 * q1] = XB[q1];
   }
 }
+
+// step 3 with the row store
+PC_HD void f512_fwd_p3(int lane, const float2* S, const float2* tab, float2* X) {
+  float2 XA[8], XB[8];
+  f512_fwd_p3_core(lane, S, tab, XA, XB);
+  f512_fwd_store(lane, XA, XB, X);
+}
+
+// Time-line tiles of the forward transform (k_fwd_fft512_lines): 16 consecutive blocks, one aligned 64-byte run of
+// every line component.  Tile [re / im][512 bins][16 samples]: a bin's 16 samples are one 64-byte row, XOR-swizzled by
+// bits 1-4 of the bin so that step 3's stores (32 consecutive bins at one sample) and the run reads (16 samples of two
+// adjacent bins) are both free of bank conflicts
+constexpr int kF512_LineR = 16;
+PC_HD int f512_lt(int k, int t) { return k * kF512_LineR + (t ^ ((k >> 1) & 15)); }
 
 // ---------------------------------------------------------------------------------------------------------
 // inverse: W[k] = Yt[k] + (-1)^k Yp[k]  (frequency-domain overlap-add), un-split, inverse steps, first half of the output
@@ -346,6 +365,82 @@ __global__ void __launch_bounds__(256, 4) k_fwd_fft512(FwdParams P, const float2
     __syncwarp();
     f512_fwd_p3(lane, S, tab, P.dst + (long long)c * P.dst_cstride + (P.dst_row0 + blk) * (long long)kF512_M);
     __syncwarp();
+  }
+}
+
+// Time-line mode (P.lines): block b goes to sample tau = line_tau0 + b of the 2 x 512 FP32 time lines of its channel,
+// which the tensor-core sweep reads, instead of through an X row and k_tc_split_x.  The CTA owns tiles of 16 samples
+// aligned to 16 in tau (the first and the last tile of the group partial): warp w transforms the blocks at samples
+// w and w + 8 of the tile with k_fwd_fft512's arithmetic, leaves the spectra in the tile (f512_lt), and the CTA then
+// stores every (line, component) run of the tile as one 64-byte piece, two runs per warp instruction.
+// grid (min(tiles, 2 * SMs / C), C), block (32, 8); dynamic smem = (1088 + 8 * 512 + 8192) float2 = 107008 bytes
+__global__ void __launch_bounds__(256, 2) k_fwd_fft512_lines(FwdParams P, const float2* __restrict__ tab512) {
+  extern __shared__ float2 pc_smem512[];
+  float2* tab = pc_smem512;
+  float2* S = pc_smem512 + kF512_TabLen + threadIdx.y * kF512_Xch;
+  float* Tre = reinterpret_cast<float*>(pc_smem512 + kF512_TabLen + 8 * kF512_Xch);
+  float* Tim = Tre + kF512_M * kF512_LineR;
+  const int lane = threadIdx.x, wid = threadIdx.y, tid = wid * 32 + lane;
+  for (int j = tid; j < kF512_TabLen; j += 256) tab[j] = tab512[j];
+  __syncthreads();
+  const int c = blockIdx.y;
+  const long long nv_total = P.nvalid_c ? (long long)P.nvalid_c[c] : P.nvalid;
+  const float* src_c = P.src + (long long)(P.use_cmap ? P.cmap[c] : c) * P.src_cstride;
+  const long long tile0 = P.line_tau0 / kF512_LineR;
+  const int ntiles = (int)((P.line_tau0 + P.nblocks - 1) / kF512_LineR - tile0 + 1);
+  // block at sample w + 8 h of tile ti (outside [0, nblocks) in the partial tiles)
+  auto block_of = [&](int ti, int h) { return (int)((tile0 + ti) * kF512_LineR - P.line_tau0) + wid + 8 * h; };
+  auto issue = [&](int blk, float2* a) {
+    if (blk < 0 || blk >= P.nblocks) return;
+    const long long rem = nv_total - (long long)blk * kF512_M;
+    const int nv = rem <= 0 ? 0 : (rem > kF512_M ? kF512_M : (int)rem);
+    const float* src = src_c + (long long)blk * kF512_M;
+    const bool vec = nv == kF512_M && (reinterpret_cast<size_t>(src) & 7) == 0;
+    f512_fwd_load(lane, src, nv, vec, a);
+  };
+  float2 nxt[8];
+  if ((int)blockIdx.x < ntiles) issue(block_of(blockIdx.x, 0), nxt);
+  for (int ti = blockIdx.x; ti < ntiles; ti += gridDim.x) {
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+      const int blk = block_of(ti, h);
+      float2 cur[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) cur[j] = nxt[j];
+      // software pipeline as in k_fwd_fft512: the warp's next block, in this tile or the next one
+      if (h == 0) issue(block_of(ti, 1), nxt);
+      else if (ti + (int)gridDim.x < ntiles) issue(block_of(ti + gridDim.x, 0), nxt);
+      if (blk < 0 || blk >= P.nblocks) continue;
+      f512_fwd_p1(lane, cur, S, tab);
+      __syncwarp();
+      float2 A[8], B[8];
+      f512_mid_load<false>(lane, S, tab, A, B);
+      __syncwarp();
+      f512_mid_store<false>(lane, S, A, B);
+      __syncwarp();
+      f512_fwd_p3_core(lane, S, tab, A, B);
+      const int t = wid + 8 * h, la = f512_la(lane), lb = f512_lb(lane);
+#pragma unroll
+      for (int q1 = 0; q1 < 8; ++q1) {
+        Tre[f512_lt(la + 64 * q1, t)] = A[q1].x; Tim[f512_lt(la + 64 * q1, t)] = A[q1].y;
+        Tre[f512_lt(lb + 64 * q1, t)] = B[q1].x; Tim[f512_lt(lb + 64 * q1, t)] = B[q1].y;
+      }
+      if (blk >= P.xrow_from)
+        f512_fwd_store(lane, A, B, P.dst + (long long)c * P.dst_cstride + (P.dst_row0 + blk) * (long long)kF512_M);
+      __syncwarp();
+    }
+    __syncthreads();                    // the tile is complete
+    const int t = lane & 15;
+    const long long tau = (tile0 + ti) * kF512_LineR + t;
+    if (tau >= P.line_tau0 && tau < P.line_tau0 + P.nblocks) {
+      const long long line0 = (long long)c * kF512_M;
+#pragma unroll 4
+      for (int k = 2 * wid + (lane >> 4); k < kF512_M; k += 16) {
+        P.lines[tc::xf_index(line0 + k, 0, tau, P.line_rows)] = Tre[f512_lt(k, t)];
+        P.lines[tc::xf_index(line0 + k, 1, tau, P.line_rows)] = Tim[f512_lt(k, t)];
+      }
+    }
+    __syncthreads();                    // the tile's reads are done before the next tile's blocks are written into it
   }
 }
 

@@ -196,21 +196,35 @@ struct SplitXParams {
   int B;
   int rows;                 // 64-sample rows per time line
   float* Xt;
+  // samples in [skip_lo, skip_hi) are left alone (the B = 512 forward FFT wrote them: k_fwd_fft512_lines).  The grid
+  // covers the 32-sample chunks 0 ... nchunk_lo - 1 and chunk_hi ... rows * 2 - 1 (split_x_chunks)
+  long long skip_lo, skip_hi;
+  int nchunk_lo, chunk_hi;
 };
 
-// grid (rows * 2, B / 32, C), block (32, 8)
+// the chunks of 32 samples a split has to visit: [0, *nlo) and [*hi, rows * 2)
+PC_TC_HD void split_x_chunks(int rows, long long skip_lo, long long skip_hi, int* nlo, int* hi) {
+  *nlo = (int)((skip_lo + 31) / 32);
+  *hi = (int)(skip_hi / 32) > *nlo ? (int)(skip_hi / 32) : *nlo;
+  if (*hi > rows * 2) *hi = rows * 2;
+}
+
+// grid (nchunk_lo + rows * 2 - chunk_hi, B / 32, C), block (32, 8)
 __global__ void __launch_bounds__(256) k_tc_split_x(SplitXParams p) {
   __shared__ float2 tile[32][33];
   const int tx = threadIdx.x, ty = threadIdx.y;
-  const long long tau0 = (long long)blockIdx.x * 32;
+  const int chunk = (int)blockIdx.x < p.nchunk_lo ? (int)blockIdx.x : p.chunk_hi + ((int)blockIdx.x - p.nchunk_lo);
+  const long long tau0 = (long long)chunk * 32;
   const int k0 = blockIdx.y * 32, ch = blockIdx.z;
   for (int r = ty; r < 32; r += 8) {
     const long long row = p.row_base + tau0 + r;
+    const bool skip = tau0 + r >= p.skip_lo && tau0 + r < p.skip_hi;
     float2 v = make_float2(0.0f, 0.0f);
-    if (row >= p.row_lo && row < p.row_hi) v = p.X[(long long)ch * p.x_cstride + row * p.B + k0 + tx];
+    if (!skip && row >= p.row_lo && row < p.row_hi) v = p.X[(long long)ch * p.x_cstride + row * p.B + k0 + tx];
     tile[r][tx] = v;
   }
   __syncthreads();
+  if (tau0 + tx >= p.skip_lo && tau0 + tx < p.skip_hi) return;
   for (int kk = ty; kk < 32; kk += 8) {
     const float2 v = tile[tx][kk];
     const long long line = (long long)ch * p.B + k0 + kk;
