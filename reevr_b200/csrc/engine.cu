@@ -572,12 +572,17 @@ void launch_cmac_bs(b200conv* h, const pc::CmacParams& P, int C) {
 constexpr int kStreamNBS = 4;      // blocks per launch the streaming sweep handles
 constexpr int kStreamPW = 8;       // warps per CTA, each striding over the CTA's partition slice
 
-int launch_cmac_stream(b200conv* h, const pc::CmacParams& P, int C) {
+pc::StreamParams stream_params(const pc::CmacParams& P) {
   pc::StreamParams S{};
   S.H = P.H; S.h_cstride = P.h_cstride;
   S.X = P.X; S.x_cstride = P.x_cstride; S.xrow0 = P.xrow0;
   S.Y = P.Y; S.y_cstride = P.y_cstride; S.y_rstride = P.y_rstride; S.yrow0 = P.yrow0;
   S.B = P.B; S.P = P.Ppad; S.nblocks = P.nblocks;
+  return S;
+}
+
+int launch_cmac_stream(b200conv* h, const pc::CmacParams& P, int C) {
+  pc::StreamParams S = stream_params(P);
   const int ktiles = (P.B / 2 + 31) / 32;
   // enough CTAs for ~2 per SM, but at least kStreamPW*4 partitions per CTA
   int nsplit = std::max(1, (2 * h->n_sm) / std::max(1, ktiles * C));
@@ -612,11 +617,7 @@ void launch_stream_rows_t(b200conv* h, const pc::StreamParams& S, dim3 grid, int
 
 // row-walking streaming sweep (B >= 64): see k_cmac_stream_rows
 int launch_cmac_stream_rows(b200conv* h, const pc::CmacParams& P, int C) {
-  pc::StreamParams S{};
-  S.H = P.H; S.h_cstride = P.h_cstride;
-  S.X = P.X; S.x_cstride = P.x_cstride; S.xrow0 = P.xrow0;
-  S.Y = P.Y; S.y_cstride = P.y_cstride; S.y_rstride = P.y_rstride; S.yrow0 = P.yrow0;
-  S.B = P.B; S.P = P.Ppad; S.nblocks = P.nblocks;
+  pc::StreamParams S = stream_params(P);
   const int threads = std::min(256, P.B / 2);
   const int xt = (P.B / 2 + threads - 1) / threads;
   // ~3 CTAs per SM, but no CTA with fewer than 8 partitions (one unrolled load batch)
@@ -677,11 +678,8 @@ struct TailXch { float2* dst; unsigned int* flag; unsigned int epoch; };
 
 int launch_cmac_stream_tma(b200conv* h, const pc::CmacParams& P, int C, int stages, int per_sm, bool dynamic = false, float skew = -1.0f,
                            const TailXch* xch = nullptr) {
-  pc::StreamParams S{};
-  S.H = P.H; S.h_cstride = P.h_cstride;
-  S.X = P.X; S.x_cstride = P.x_cstride; S.xrow0 = P.xrow0;
-  S.Y = P.Y; S.y_cstride = P.y_cstride; S.y_rstride = P.y_rstride; S.yrow0 = P.yrow0;
-  S.B = P.B; S.P = P.Ppad; S.nblocks = 1;
+  pc::StreamParams S = stream_params(P);
+  S.nblocks = 1;
   const int W = pc::stream_tma_w(P.B), PP = pc::stream_tma_pp(P.B), RG = pc::stream_tma_rg(P.B);
   const int xt = P.B / W;
   // per_sm CTAs per SM, but no CTA with fewer than two ring stages of partitions
@@ -1232,11 +1230,6 @@ int copy_in(b200conv* h, float* dst, size_t dstride, const float* src, size_t ss
   return 0;
 }
 
-void set_cmap(const b200conv* h, pc::FwdParams& fp, bool direct) {
-  fp.use_cmap = (direct && (h->route_on || h->route_in_only)) ? 1 : 0;
-  for (int c = 0; c < 8; ++c) fp.cmap[c] = h->in_map[c];
-}
-
 #if !defined(PC_EMULATE)
 #define PC_LAUNCH_MIX(mp, grid, st) pc::k_mix<<<grid, 256, 0, st>>>(mp)
 #endif
@@ -1276,6 +1269,80 @@ int compact_timeline(b200conv* h, Stage& s) {
     CU_CHECK(h, cudaMemcpyAsync(base, base + (size_t)(s.head - s.hist) * B, bytes, cudaMemcpyDeviceToDevice, h->s_launch));
   }
   s.head = s.hist;
+  return 0;
+}
+
+// room for nb more X rows from the open block on (plus the sweeps' slack rows)
+int ensure_rows(b200conv* h, Stage& s, int nb) {
+  return s.head + nb + kMaxTT > s.R ? compact_timeline(h, s) : 0;
+}
+
+// How a Stage maps onto the kernels' parameter blocks.  The sweep of `nblocks` blocks from the open one on writes Y
+// rows 1..; with `extra` it starts that many blocks early (row 0, see run_group).
+pc::CmacParams sweep_params(const Stage& s, int C, float2* Y, int nblocks, int extra = 0) {
+  pc::CmacParams cp{};
+  cp.H = s.H; cp.h_cstride = (long long)s.Prows * s.B;
+  cp.X = s.X; cp.x_cstride = (long long)s.R * s.B; cp.xrow0 = s.head - s.p_begin - extra;
+  cp.Y = Y; cp.y_cstride = s.B; cp.y_rstride = (long long)C * s.B; cp.yrow0 = 1 - extra;
+  cp.B = s.B; cp.Ppad = s.P; cp.nblocks = nblocks + extra;
+  return cp;
+}
+
+// forward FFT of `nblocks` blocks (`nvalid` samples, zero-padded) into the X rows from the open block on; `direct`: src
+// is the caller's buffer, whose channels go through the input routing
+pc::FwdParams fwd_params(const b200conv* h, const Stage& s, const float* src, size_t src_stride, long long nvalid,
+                         int nblocks, bool direct) {
+  pc::FwdParams fp{};
+  fp.src = src; fp.src_cstride = (long long)src_stride;
+  fp.nvalid_c = nullptr; fp.nvalid = nvalid;
+  fp.use_cmap = (direct && (h->route_on || h->route_in_only)) ? 1 : 0;
+  for (int c = 0; c < 8; ++c) fp.cmap[c] = h->in_map[c];
+  fp.dst = s.X; fp.dst_cstride = (long long)s.R * s.B; fp.dst_row0 = s.head;
+  fp.tw = s.tw; fp.tab512 = s.tab512; fp.M = s.B; fp.nblocks = nblocks;
+  return fp;
+}
+
+// inverse FFT of Y rows 1..nblocks (row 0 is the overlap state); the caller adds the destination
+pc::InvParams inv_params(const Stage& s, int C, float2* Y, int nblocks) {
+  pc::InvParams ip{};
+  ip.Y = Y; ip.y_cstride = s.B; ip.y_rstride = (long long)C * s.B; ip.yrow0 = 1;
+  ip.tw = s.tw; ip.tab512 = s.tab512; ip.M = s.B; ip.nblocks = nblocks; ip.scale = 1.0f / (float)s.B;
+  return ip;
+}
+
+// ... into the look-ahead ring of a stage >= 1, q blocks ahead of the stage's input
+void inv_into_ring(pc::InvParams& ip, const Stage& s) {
+  ip.dst = s.fut; ip.dst_cstride = (long long)s.ring;
+  ip.index0 = (s.blocks_done + s.q) * (long long)s.B;
+  ip.lo = 0; ip.hi = (long long)1 << 62; ip.mask = (long long)s.ring - 1;
+}
+
+// How the n samples of a launch group enter a stage's open block: `complete` blocks to transform from `src`, `partial`
+// samples left over as the next open block.
+struct Intake { int complete, partial; bool direct; const float* src; size_t src_stride; size_t total; };
+
+// With an empty open block the forward FFT reads the caller's buffer directly; only a trailing partial block is
+// buffered.  Otherwise the new samples are appended behind the open block's.
+int intake_begin(b200conv* h, Stage& s, const float* in_dev, size_t in_stride, size_t n, Intake* it) {
+  it->total = (size_t)s.fill + n;
+  it->complete = (int)(it->total / s.B);
+  it->partial = (int)(it->total % s.B);
+  it->direct = s.fill == 0;
+  it->src = it->direct ? in_dev : s.inbuf;
+  it->src_stride = it->direct ? in_stride : s.in_stride;
+  return it->direct ? 0 : copy_in(h, s.inbuf + s.fill, s.in_stride, in_dev, in_stride, n);
+}
+
+// the trailing partial block goes to the front of inbuf (with nothing completed and samples appended it is there already)
+int intake_end(b200conv* h, Stage& s, const Intake& it) {
+  const size_t off = (size_t)it.complete * s.B;
+  if (it.partial > 0 && it.direct) {
+    if (int rc = copy_in(h, s.inbuf, s.in_stride, it.src + off, it.src_stride, it.partial)) return rc;
+  } else if (it.partial > 0 && it.complete > 0) {
+    CU_CHECK(h, cudaMemcpy2DAsync(s.inbuf, s.in_stride * sizeof(float), s.inbuf + off, s.in_stride * sizeof(float),
+                                  it.partial * sizeof(float), h->C, cudaMemcpyDeviceToDevice, h->s_main));
+  }
+  s.fill = it.partial;
   return 0;
 }
 
@@ -1503,33 +1570,27 @@ int launch_sum_slots(b200conv* h, float2* dst, const float2* src, size_t n, int 
   return 0;
 }
 
-// One completed block of a stage >= 1 of a tail-sharded handle, spectrum in X row s.head (output block s.blocks_done),
-// everything on h->s_launch: the sweep over this rank's partitions, the partial spectra of all ranks summed on rank 0
-// (slot exchange, else the reduce hook), and on rank 0 the inverse FFT into the stage's look-ahead ring.
+// One completed block of a stage >= 1, spectrum in X row s.head (output block s.blocks_done), everything on
+// h->s_launch: the sweep over this rank's partitions, on a tail-sharded handle the partial spectra of all ranks summed
+// on rank 0 (slot exchange, else the reduce hook), and on rank 0 (the only rank of an unsharded handle) the inverse
+// FFT into the stage's look-ahead ring.
 int tail_block(b200conv* h, Stage& s, int si) {
   const int C = h->C, B = s.B, G = h->cfg.shard_count, g = h->cfg.shard_rank;
   const size_t row = (size_t)C * B;
   cudaStream_t st = h->s_launch;
   float2* Yb = s.Y[s.ybuf];
-  pc::CmacParams cp{};
-  cp.H = s.H; cp.h_cstride = (long long)s.Prows * B;
-  cp.X = s.X; cp.x_cstride = (long long)s.R * B; cp.xrow0 = s.head - s.p_begin;
-  cp.Y = Yb; cp.y_cstride = B; cp.y_rstride = (long long)row; cp.yrow0 = 1;
-  cp.B = B; cp.Ppad = s.P; cp.nblocks = 1;
-  pc::InvParams ip{};
-  ip.y_cstride = B; ip.y_rstride = (long long)row; ip.yrow0 = 1;
-  ip.tw = s.tw; ip.tab512 = s.tab512; ip.M = B; ip.nblocks = 1; ip.scale = 1.0f / (float)B;
-  ip.dst = s.fut; ip.dst_cstride = (long long)s.ring;
-  ip.index0 = (s.blocks_done + s.q) * (long long)B;
-  ip.lo = 0; ip.hi = (long long)1 << 62; ip.mask = (long long)s.ring - 1;
-  if (!h->p2p_tail) {                       // reduce hook: once per tail block, never for the head
+  const pc::CmacParams cp = sweep_params(s, C, Yb, 1);
+  pc::InvParams ip = inv_params(s, C, Yb, 1);
+  inv_into_ring(ip, s);
+  if (!h->p2p_tail) {
     if (s.P > 0) { if (int rc = launch_cmac(h, cp, C)) return rc; }
     else CU_CHECK(h, cudaMemsetAsync(Yb + row, 0, row * sizeof(float2), st));
-    if (!h->reduce) return fail(h, B200CONV_ESTATE, "sharded handle without a reduce hook");
-    if (h->reduce(h->reduce_user, reinterpret_cast<float*>(Yb + row), row * 2, st) != 0)
-      return fail(h, B200CONV_ECUDA, "reduce hook failed");
+    if (tail_layout(h)) {                   // reduce hook: once per tail block, never for the head
+      if (!h->reduce) return fail(h, B200CONV_ESTATE, "sharded handle without a reduce hook");
+      if (h->reduce(h->reduce_user, reinterpret_cast<float*>(Yb + row), row * 2, st) != 0)
+        return fail(h, B200CONV_ECUDA, "reduce hook failed");
+    }
     if (g == 0) {
-      ip.Y = Yb;
       if (int rc = launch_inv(h, ip, C, st)) return rc;
       CU_CHECK(h, cudaMemcpyAsync(Yb, Yb + row, row * sizeof(float2), cudaMemcpyDeviceToDevice, st));   // overlap state
     }
@@ -1560,37 +1621,19 @@ int run_tail_stages(b200conv* h, const float* in_dev, size_t in_stride, size_t n
   const int C = h->C;
   for (size_t si = 1; si < h->stages.size(); ++si) {
     Stage& s = h->stages[si];
-    const int B = s.B;
-    const size_t total = (size_t)s.fill + n;
-    const int complete = (int)(total / B);
-    const int partial = (int)(total % B);
-    const bool direct = (s.fill == 0);
-    if (!direct) { if (int rc = copy_in(h, s.inbuf + s.fill, s.in_stride, in_dev, in_stride, n)) return rc; }
-    if (complete > 0) {
-      if (s.head + complete + kMaxTT > s.R) { if (int rc = compact_timeline(h, s)) return rc; }
-      pc::FwdParams fp{};
-      fp.src = direct ? in_dev : s.inbuf;
-      fp.src_cstride = direct ? (long long)in_stride : (long long)s.in_stride;
-      fp.nvalid_c = nullptr; fp.nvalid = (long long)total;
-      set_cmap(h, fp, direct);
-      fp.dst = s.X; fp.dst_cstride = (long long)s.R * B; fp.dst_row0 = s.head;
-      fp.tw = s.tw; fp.tab512 = s.tab512; fp.M = B; fp.nblocks = complete;
+    Intake it;
+    if (int rc = intake_begin(h, s, in_dev, in_stride, n, &it)) return rc;
+    if (it.complete > 0) {
+      if (int rc = ensure_rows(h, s, it.complete)) return rc;
+      const pc::FwdParams fp = fwd_params(h, s, it.src, it.src_stride, (long long)it.total, it.complete, it.direct);
       if (int rc = launch_fwd(h, fp, C)) return rc;
-      for (int j = 0; j < complete; ++j) {
+      for (int j = 0; j < it.complete; ++j) {
         if (int rc = tail_block(h, s, (int)si)) return rc;
         s.head += 1;
         s.blocks_done += 1;
       }
-      if (partial > 0) {
-        if (direct) { if (int rc = copy_in(h, s.inbuf, s.in_stride, in_dev + (size_t)complete * B, in_stride, partial)) return rc; }
-        else
-          CU_CHECK(h, cudaMemcpy2DAsync(s.inbuf, s.in_stride * sizeof(float), s.inbuf + (size_t)complete * B,
-                                        s.in_stride * sizeof(float), partial * sizeof(float), C, cudaMemcpyDeviceToDevice, h->s_main));
-      }
-    } else if (direct && partial > 0) {
-      if (int rc = copy_in(h, s.inbuf, s.in_stride, in_dev, in_stride, partial)) return rc;
     }
-    s.fill = partial;
+    if (int rc = intake_end(h, s, it)) return rc;
   }
   return 0;
 }
@@ -1604,32 +1647,21 @@ int run_group_p2p(b200conv* h, const float* in_dev, size_t in_stride, float* out
   cudaStream_t ps = h->s_post;
   if (n == 0) return 0;
   if (n + B > h->Lmax) return fail(h, B200CONV_ESTATE, "launch group larger than the staging buffers");
-  const size_t total = (size_t)s.fill + n;
-  const int complete = (int)(total / B);
-  const int partial = (int)(total % B);
-  const int nb = complete + (partial > 0 ? 1 : 0);
-  const bool direct = (s.fill == 0);
-  if (!direct)
-    CU_CHECK(h, cudaMemcpy2DAsync(s.inbuf + s.fill, s.in_stride * sizeof(float), in_dev, in_stride * sizeof(float),
-                                  n * sizeof(float), C, cudaMemcpyDeviceToDevice, h->s_main));
+  Intake it;
+  if (int rc = intake_begin(h, s, in_dev, in_stride, n, &it)) return rc;
+  const int complete = it.complete;
+  const int nb = complete + (it.partial > 0 ? 1 : 0);
   const int yb = s.ybuf;
   const int per = (nb + G - 1) / G;
-  if (s.head + nb + kMaxTT > s.R) { if (int rc = compact_timeline(h, s)) return rc; }
-  pc::FwdParams fp{};
-  fp.src = direct ? in_dev : s.inbuf;
-  fp.src_cstride = direct ? (long long)in_stride : (long long)s.in_stride;
-  fp.nvalid_c = nullptr; fp.nvalid = (long long)total;
-  fp.dst = s.X; fp.dst_cstride = (long long)s.R * B; fp.dst_row0 = s.head;
-  fp.tw = s.tw; fp.tab512 = s.tab512; fp.M = B; fp.nblocks = nb;
+  if (int rc = ensure_rows(h, s, nb)) return rc;
+  // (routing is refused on this path: the input map stays unused)
+  const pc::FwdParams fp = fwd_params(h, s, it.src, it.src_stride, (long long)it.total, nb, it.direct);
   if (int rc = launch_fwd(h, fp, C)) return rc;
 
   // the exchange buffers of parity yb are free once every GPU finished the inverse FFT of two groups ago
   CU_CHECK(h, cudaStreamWaitEvent(h->s_main, s.ev_post[yb], 0));
-  pc::CmacParams cp{};
-  cp.H = s.H; cp.h_cstride = (long long)s.Prows * B;
-  cp.X = s.X; cp.x_cstride = (long long)s.R * B; cp.xrow0 = s.head - s.p_begin;
-  cp.Y = nullptr; cp.y_cstride = B; cp.y_rstride = (long long)row; cp.yrow0 = 0;
-  cp.B = B; cp.Ppad = s.P; cp.nblocks = nb;
+  pc::CmacParams cp = sweep_params(s, C, nullptr, nb);    // the rows go to the ranks' exchange slots
+  cp.yrow0 = 0;
   cp.xg = G; cp.xrank = g; cp.xper = per; cp.xslot = (long long)h->xslot;
   cp.xhalo_block = complete > 0 ? complete - 1 : -1;
   for (int r = 0; r < G; ++r) cp.xbase[r] = h->peerYx[r][yb];
@@ -1648,13 +1680,10 @@ int run_group_p2p(b200conv* h, const float* in_dev, size_t in_stride, float* out
       if (int rc = copy_rows_kernel(h, reinterpret_cast<float*>(h->Yx[yb]), h->xslot * 2,
                                     reinterpret_cast<const float*>(h->Hh + (size_t)h->hidx * G * row), row * 2, row * 2, G, ps)) return rc;
     }
-    pc::InvParams ip{};
-    ip.Y = h->Yx[yb]; ip.y_cstride = B; ip.y_rstride = (long long)row; ip.yrow0 = 1;
-    ip.tw = s.tw; ip.tab512 = s.tab512; ip.M = B; ip.nblocks = j1 - j0; ip.scale = 1.0f / (float)B;
+    pc::InvParams ip = inv_params(s, C, h->Yx[yb], j1 - j0);
     ip.n_partials = G; ip.partial_stride = (long long)h->xslot;
     ip.dst = h->peer_xout0[yb]; ip.dst_cstride = (long long)h->Lmax;
     ip.index0 = -(long long)s.fill + (long long)j0 * B; ip.lo = 0; ip.hi = (long long)n; ip.mask = -1;
-    ip.n_add = 0; ip.abs0 = 0;
     if (int rc = launch_inv(h, ip, C, ps)) return rc;
   }
   if (int rc = p2p_barrier(h, ps)) return rc;          // every slice of the audio is in shard 0's exchange buffer
@@ -1666,19 +1695,10 @@ int run_group_p2p(b200conv* h, const float* in_dev, size_t in_stride, float* out
   if (complete > 0) {
     s.ybuf = yb ^ 1;
     h->hidx = (h->hidx + 1) % 3;
-    if (partial > 0) {
-      const float* tail_src = direct ? in_dev + (size_t)complete * B : s.inbuf + (size_t)complete * B;
-      const size_t tail_pitch = direct ? in_stride : s.in_stride;
-      CU_CHECK(h, cudaMemcpy2DAsync(s.inbuf, s.in_stride * sizeof(float), tail_src, tail_pitch * sizeof(float),
-                                    partial * sizeof(float), C, cudaMemcpyDeviceToDevice, h->s_main));
-    }
     s.head += complete;
     s.blocks_done += complete;
-  } else if (direct && partial > 0) {
-    CU_CHECK(h, cudaMemcpy2DAsync(s.inbuf, s.in_stride * sizeof(float), in_dev, in_stride * sizeof(float),
-                                  partial * sizeof(float), C, cudaMemcpyDeviceToDevice, h->s_main));
   }
-  s.fill = partial;
+  if (int rc = intake_end(h, s, it)) return rc;
   h->abs_pos += (long long)n;
   return 0;
 }
@@ -1712,14 +1732,10 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
     Stage& s = h->stages[si];
     const int B = s.B;
     const size_t row = (size_t)C * B;           // float2 per Y row (all channels)
-    const size_t total = (size_t)s.fill + n;
-    const int complete = (int)(total / B);
-    const int partial = (int)(total % B);
-    const int nb = (si == 0) ? complete + (partial > 0 ? 1 : 0) : complete;
-    // With an empty open block the forward FFT reads the caller's buffer directly; only a trailing
-    // partial block is buffered.  Otherwise the new samples are appended behind the open block's.
-    const bool direct = (s.fill == 0);
-    if (!direct) { if (int rc = copy_in(h, s.inbuf + s.fill, s.in_stride, in_dev, in_stride, n)) return rc; }
+    Intake it;
+    if (int rc = intake_begin(h, s, in_dev, in_stride, n, &it)) return rc;
+    const int complete = it.complete;
+    const int nb = (si == 0) ? complete + (it.partial > 0 ? 1 : 0) : complete;
     const int yb = s.ybuf;
     float2* Yb = s.Y[yb];
     // B = 512 groups on the tensor-core sweep (unsharded): the inverse FFT reads the sweep's bin-major result
@@ -1728,28 +1744,18 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
     TcDirect td{};
     long long yc_stride = 0;
     if (nb > 0) {
-      if (s.head + nb + kMaxTT > s.R) { if (int rc = compact_timeline(h, s)) return rc; }
+      if (int rc = ensure_rows(h, s, nb)) return rc;
       // overlap state after a forward-FFT-only advance (time-slice sharding): Y row 0 must become
       // sum_p H[p] X[head-1-p], the spectrum of the block in front of this group — its input spectra are in the
       // timeline, so the sweep simply starts one block early and writes that block as row 0
       const int extra = (si == 0 && h->yprev_stale) ? 1 : 0;
-      pc::CmacParams cp{};
-      cp.H = s.H; cp.h_cstride = (long long)s.Prows * B;
-      cp.X = s.X; cp.x_cstride = (long long)s.R * B; cp.xrow0 = s.head - s.p_begin - extra;
-      cp.Y = Yb; cp.y_cstride = B; cp.y_rstride = (long long)row; cp.yrow0 = 1 - extra;
-      cp.B = B; cp.Ppad = s.P; cp.nblocks = nb + extra;
+      const pc::CmacParams cp = sweep_params(s, C, Yb, nb, extra);
       const bool direct_ok = h->cfg.shard_count == 1 && use_fft512(h, B, nb, C, s.tab512);
       int variant = 0;
       if (int rc = select_cmac(h, cp, C, direct_ok ? &s.tcY[yb] : nullptr, &s.tcY_bytes[yb], &variant)) return rc;
       tc_direct = direct_ok && variant == 40;
 
-      pc::FwdParams fp{};
-      fp.src = direct ? in_dev : s.inbuf;
-      fp.src_cstride = direct ? (long long)in_stride : (long long)s.in_stride;
-      fp.nvalid_c = nullptr; fp.nvalid = (long long)total;
-      set_cmap(h, fp, direct);
-      fp.dst = s.X; fp.dst_cstride = (long long)s.R * B; fp.dst_row0 = s.head;
-      fp.tw = s.tw; fp.tab512 = s.tab512; fp.M = B; fp.nblocks = nb;
+      pc::FwdParams fp = fwd_params(h, s, it.src, it.src_stride, (long long)it.total, nb, it.direct);
       if (tc_direct) {
         td.Yc = s.tcY[yb]; td.extra = extra;
         const pc::tc::Geom tg = pc::tc::make_geom(cp.Ppad, cp.nblocks);
@@ -1782,9 +1788,7 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
           return fail(h, B200CONV_ECUDA, "reduce hook failed");
       }
       if (root) {
-        pc::InvParams ip{};
-        ip.Y = Yb; ip.y_cstride = B; ip.y_rstride = (long long)row; ip.yrow0 = 1;
-        ip.tw = s.tw; ip.tab512 = s.tab512; ip.M = B; ip.nblocks = nb; ip.scale = 1.0f / (float)B;
+        pc::InvParams ip = inv_params(s, C, Yb, nb);
         if (tc_direct) {   // block t at slot kYLead + extra + t; block -1 is the overlap state (Y row 0) unless swept
           ip.yc = td.Yc; ip.yc_stride = yc_stride; ip.yc_slot0 = pc::tc::kYLead + td.extra;
           ip.yc_prev_row = td.extra == 0;
@@ -1802,10 +1806,7 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
           }
           ip.n_add = na;
         } else {
-          ip.dst = s.fut; ip.dst_cstride = (long long)s.ring;
-          ip.index0 = (s.blocks_done + s.q) * (long long)B;
-          ip.lo = 0; ip.hi = (long long)1 << 62; ip.mask = (long long)s.ring - 1;
-          ip.n_add = 0; ip.abs0 = 0;
+          inv_into_ring(ip, s);
         }
         if (int rc = launch_inv(h, ip, C, ps)) return rc;
         if (si == 0 && h->route_on) { if (int rc = launch_mix(h, h->dch[0], h->Lmax, out_dev, out_stride, n, ps)) return rc; }
@@ -1823,21 +1824,12 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
                                     cudaMemcpyDeviceToDevice, ps));
       if (overlap) CU_CHECK(h, cudaEventRecord(s.ev_post[yb], ps));
       s.ybuf = nxt;
-      if (partial > 0) {
-        if (direct) { if (int rc = copy_in(h, s.inbuf, s.in_stride, in_dev + (size_t)complete * B, in_stride, partial)) return rc; }
-        else
-          CU_CHECK(h, cudaMemcpy2DAsync(s.inbuf, s.in_stride * sizeof(float), s.inbuf + (size_t)complete * B,
-                                        s.in_stride * sizeof(float), partial * sizeof(float), C, cudaMemcpyDeviceToDevice, h->s_main));
-      }
       s.head += complete;
       s.blocks_done += complete;
-    } else {
-      if (direct && partial > 0) {   // nothing completed: keep the partial block's samples for the next call
-        if (int rc = copy_in(h, s.inbuf, s.in_stride, in_dev, in_stride, partial)) return rc;
-      }
-      if (overlap && nb > 0) CU_CHECK(h, cudaEventRecord(s.ev_post[yb], ps));
     }
-    s.fill = partial;
+    if (int rc = intake_end(h, s, it)) return rc;
+    // a group that completed no block releases Y[yb] here (one that did, above)
+    if (complete == 0 && overlap && nb > 0) CU_CHECK(h, cudaEventRecord(s.ev_post[yb], ps));
   }
   h->abs_pos += (long long)n;
   return 0;
@@ -1851,13 +1843,8 @@ int advance_fft_only(b200conv* h, const float* in_dev, size_t in_stride, long lo
   const int C = h->C, B = s.B;
   for (long long done = 0; done < nblocks;) {
     const int nb = (int)std::min<long long>(nblocks - done, s.Tcap);
-    if (s.head + nb + kMaxTT > s.R) { if (int rc = compact_timeline(h, s)) return rc; }
-    pc::FwdParams fp{};
-    fp.src = in_dev + (size_t)done * B; fp.src_cstride = (long long)in_stride;
-    fp.nvalid_c = nullptr; fp.nvalid = (long long)nb * B;
-    set_cmap(h, fp, false);
-    fp.dst = s.X; fp.dst_cstride = (long long)s.R * B; fp.dst_row0 = s.head;
-    fp.tw = s.tw; fp.tab512 = s.tab512; fp.M = B; fp.nblocks = nb;
+    if (int rc = ensure_rows(h, s, nb)) return rc;
+    const pc::FwdParams fp = fwd_params(h, s, in_dev + (size_t)done * B, in_stride, (long long)nb * B, nb, false);
     if (int rc = launch_fwd(h, fp, C)) return rc;
     s.head += nb;
     s.blocks_done += nb;
@@ -1912,39 +1899,11 @@ int drain_tail(b200conv* h) {
 // ONE completed block of a stage >= 1 (its samples are in s.inbuf), everything on h->s_launch: forward FFT into the
 // timeline, streaming sweep, inverse FFT into the stage's look-ahead ring (TwoStageFFTConvolver.cpp:201-222)
 int run_tail_block(b200conv* h, Stage& s) {
-  const int C = h->C, B = s.B;
-  const size_t row = (size_t)C * B;
-  cudaStream_t st = h->s_launch;
-  if (s.head + 1 + kMaxTT > s.R) { if (int rc = compact_timeline(h, s)) return rc; }
-  pc::FwdParams fp{};
-  fp.src = s.inbuf; fp.src_cstride = (long long)s.in_stride;
-  fp.nvalid_c = nullptr; fp.nvalid = (long long)B;
-  fp.dst = s.X; fp.dst_cstride = (long long)s.R * B; fp.dst_row0 = s.head;
-  fp.tw = s.tw; fp.tab512 = s.tab512; fp.M = B; fp.nblocks = 1;
-  if (int rc = launch_fwd(h, fp, C)) return rc;
-  if (tail_layout(h)) {            // rank 0 of a tail-sharded handle: the other ranks' partial spectra join here
-    if (int rc = tail_block(h, s, (int)(&s - h->stages.data()))) return rc;
-    s.head += 1;
-    s.blocks_done += 1;
-    s.fill = 0;
-    return 0;
-  }
-  float2* Yb = s.Y[s.ybuf];
-  pc::CmacParams cp{};
-  cp.H = s.H; cp.h_cstride = (long long)s.Prows * B;
-  cp.X = s.X; cp.x_cstride = (long long)s.R * B; cp.xrow0 = s.head - s.p_begin;
-  cp.Y = Yb; cp.y_cstride = B; cp.y_rstride = (long long)row; cp.yrow0 = 1;
-  cp.B = B; cp.Ppad = s.P; cp.nblocks = 1;
-  if (int rc = launch_cmac(h, cp, C)) return rc;
-  pc::InvParams ip{};
-  ip.Y = Yb; ip.y_cstride = B; ip.y_rstride = (long long)row; ip.yrow0 = 1;
-  ip.tw = s.tw; ip.tab512 = s.tab512; ip.M = B; ip.nblocks = 1; ip.scale = 1.0f / (float)B;
-  ip.dst = s.fut; ip.dst_cstride = (long long)s.ring;
-  ip.index0 = (s.blocks_done + s.q) * (long long)B;
-  ip.lo = 0; ip.hi = (long long)1 << 62; ip.mask = (long long)s.ring - 1;
-  ip.n_add = 0; ip.abs0 = 0;
-  if (int rc = launch_inv(h, ip, C, st)) return rc;
-  CU_CHECK(h, cudaMemcpyAsync(Yb, Yb + row, row * sizeof(float2), cudaMemcpyDeviceToDevice, st));   // overlap state
+  if (int rc = ensure_rows(h, s, 1)) return rc;
+  const pc::FwdParams fp = fwd_params(h, s, s.inbuf, s.in_stride, s.B, 1, false);
+  if (int rc = launch_fwd(h, fp, h->C)) return rc;
+  // on rank 0 of a tail-sharded handle the other ranks' partial spectra join here
+  if (int rc = tail_block(h, s, (int)(&s - h->stages.data()))) return rc;
   s.head += 1;
   s.blocks_done += 1;
   s.fill = 0;
@@ -2013,7 +1972,7 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
         h->rt_tail_joined = true;
       }
   }
-  if (s0.head + 1 + kMaxTT > s0.R) { if (int rc = compact_timeline(h, s0)) return rc; }
+  if (int rc = ensure_rows(h, s0, 1)) return rc;
   pc::RtParams P{};
   P.M = M; P.C = C; P.NC = nc; P.P = s0.P;
   P.fill = s0.fill; P.len = (int)len; P.complete = (s0.fill + (int)len == M) ? 1 : 0;
@@ -2070,12 +2029,7 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
     const size_t row = (size_t)C * M;
     P.mode = 1;
     if (int rc = launch(P)) return rc;
-    pc::CmacParams cp{};
-    cp.H = s0.H; cp.h_cstride = (long long)s0.Prows * M;
-    cp.X = s0.X; cp.x_cstride = (long long)s0.R * M; cp.xrow0 = s0.head - s0.p_begin;
-    cp.Y = Yb; cp.y_cstride = M; cp.y_rstride = (long long)row; cp.yrow0 = 1;
-    cp.B = M; cp.Ppad = s0.P; cp.nblocks = 1;
-    if (int rc = launch_cmac(h, cp, C)) return rc;
+    if (int rc = launch_cmac(h, sweep_params(s0, C, Yb, 1), C)) return rc;
     P.mode = 2; P.Yt = Yb + row;
     if (use_flag && h->hflag_dev) { P.done_flag = h->hflag_dev; P.done_val = ++h->flag_epoch; }
     if (int rc = launch(P)) return rc;
@@ -2374,7 +2328,20 @@ int b200conv_process_device(b200conv_t* h, const float* in_dev, size_t in_stride
 // cannot overlap with compute, so the sequence ramps up from one sweep wave (w, 2w, 4w, ...), runs steady groups of
 // `grp` samples and ramps down again; every group but the last is a whole number of waves / 64-block tiles, the last
 // one carries whatever is left (incl. a ragged tail).
-static std::vector<size_t> ramped_groups(size_t len, size_t wave, size_t tile, size_t grp, size_t cap) {
+// Long calls are split into groups so that the PCIe copies overlap with compute: only the first group's H2D
+// and the last group's D2H are exposed, so aim for ~`parts` groups — but keep every group a whole number of
+// sweep WAVES (n_sm x 3 CTAs x 64 blocks per CTA over ceil(B/32) x C tile columns), otherwise a
+// partially filled last wave costs more than the overlap gains.  `cap` is the staging capacity; the steady group
+// size goes to *grp_out.
+static std::vector<size_t> ramped_groups(const b200conv_t* h, size_t B, size_t len, size_t parts, size_t cap,
+                                         size_t* grp_out = nullptr) {
+  const size_t tile = B * 64;
+  const size_t cols = (size_t)((B + 31) / 32) * (size_t)h->C;
+  size_t wave = ((size_t)h->n_sm * 3 * 64 + cols - 1) / cols * B;       // samples per full wave
+  wave = std::max(tile, wave / tile * tile);
+  size_t grp = std::max(wave, (len / parts) / wave * wave);
+  grp = std::min(grp, cap >= tile ? cap / tile * tile : cap);
+  if (grp_out) *grp_out = grp;
   std::vector<size_t> g, up;
   size_t tot = 0;
   for (size_t r = wave; r * 2 <= grp && 2 * (tot + r) + 2 * grp <= len; r *= 2) { up.push_back(r); tot += r; }
@@ -2485,17 +2452,7 @@ static int process_impl(b200conv_t* h, const float* const* in, float* const* out
   // throughput path: H2D / compute / D2H of successive groups overlap on three streams
   size_t done = 0;
   int i = 0;
-  // Split long calls into groups so that the PCIe copies overlap with compute: only the first group's H2D
-  // and the last group's D2H are exposed, so aim for ~8 groups — but keep every group a whole number of
-  // sweep WAVES (n_sm x 3 CTAs x 64 blocks per CTA over ceil(B/32) x C tile columns), otherwise a
-  // partially filled last wave costs more than the overlap gains.
-  const size_t tile = (size_t)B0 * 64;
-  const size_t cols = (size_t)((B0 + 31) / 32) * (size_t)h->C;
-  size_t wave = ((size_t)h->n_sm * 3 * 64 + cols - 1) / cols * (size_t)B0;       // samples per full wave
-  wave = std::max(tile, wave / tile * tile);
-  size_t grp = std::max(wave, (len / 8) / wave * wave);
-  grp = std::min(grp, chunk >= tile ? chunk / tile * tile : chunk);
-  const std::vector<size_t> groups = ramped_groups(len, wave, tile, grp, chunk);
+  const std::vector<size_t> groups = ramped_groups(h, B0, len, 8, chunk);
   for (size_t gi = 0; gi < groups.size() && done < len; ++gi, ++i) {
     const int b = i & 1;
     const size_t n = std::min(len - done, groups[gi]);
@@ -2581,13 +2538,9 @@ int b200conv_process_sliced(b200conv_t* h, const float* const* in, float* const*
   // pieces of at most `grp` samples, each one H2D -> (forward FFTs | full group) -> D2H, pipelined over the three
   // streams like b200conv_process: [lo, a) and [tail_lo, T) are transformed only, [a, b) is convolved
   const size_t chunk = (h->Lmax - B) / B * B;
-  const size_t tile = B * 64;
-  const size_t cols = (size_t)((B + 31) / 32) * (size_t)C;
-  size_t wave = ((size_t)h->n_sm * 3 * 64 + cols - 1) / cols * B;
-  wave = std::max(tile, wave / tile * tile);
   const size_t n_slice = (size_t)(sp.b - sp.a) * B;
-  size_t grp = std::max(wave, (n_slice / 4) / wave * wave);
-  grp = std::min(grp, chunk >= tile ? chunk / tile * tile : chunk);
+  size_t grp = 0;
+  const std::vector<size_t> slice_groups = ramped_groups(h, B, n_slice, 4, chunk, &grp);
   struct Piece { size_t off, n; bool conv; };
   std::vector<Piece> pieces;
   auto add = [&](long long b0, long long b1, bool conv) {
@@ -2596,7 +2549,7 @@ int b200conv_process_sliced(b200conv_t* h, const float* const* in, float* const*
   add(sp.lo, sp.a, false);
   {   // the slice itself: ramped groups (short first H2D, short last D2H)
     size_t o = (size_t)sp.a * B;
-    for (size_t gsz : ramped_groups(n_slice, wave, tile, grp, chunk)) { pieces.push_back({o, gsz, true}); o += gsz; }
+    for (size_t gsz : slice_groups) { pieces.push_back({o, gsz, true}); o += gsz; }
   }
   add(sp.tail_lo, sp.T, false);
   int i = 0;
