@@ -74,6 +74,10 @@ public:
 
   const std::string& error() const { return _error; }
 
+  // fixed-latency mode (b200conv_set_latency) of the handle; 0 without one
+  bool setLatency(size_t samples) { return ok(b200conv_set_latency(get(), samples), "setLatency"); }
+  size_t latency() const { return _h ? b200conv_latency(_h) : 0; }
+
 private:
   b200conv_t* _h;
   std::string _error;
@@ -112,6 +116,11 @@ public:
 
   // additions (not in the reference)
   const char* lastError() const { return _handle.error().c_str(); }
+  // fixed-latency mode: process() returns its output `samples` later (0, or a multiple of the block size up to 16
+  // blocks), so that the call never waits for the GPU while it keeps up; after init(), which returns to zero latency.
+  // Clears the convolver.  Report getLatency() to the host (JUCE setLatencySamples).
+  bool setLatency(size_t samples) { return _handle.setLatency(samples); }
+  size_t getLatency() const { return _handle.latency(); }
 
 private:
   detail::Handle _handle;

@@ -88,6 +88,9 @@ public:
   }
 
   const char* lastError() const { return _handle.error().c_str(); }
+  // fixed-latency mode (additions, not in the reference): see FFTConvolver::setLatency; a multiple of the head block
+  bool setLatency(size_t samples) { return _handle.setLatency(samples); }
+  size_t getLatency() const { return _handle.latency(); }
 
 protected:
   virtual void startBackgroundProcessing() { doBackgroundProcessing(); }

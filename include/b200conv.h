@@ -100,6 +100,27 @@ int b200conv_clear(b200conv_t* h);
 /* FFTConvolver::reset (FFTConvolver.cpp:56-78): drop the IR and all device memory. */
 int b200conv_reset(b200conv_t* h);
 
+/* Fixed-latency mode (beyond the reference; a plugin reports it to its host, e.g. JUCE setLatencySamples).
+ * samples = 0: zero latency (default).  Otherwise a multiple of the head block B0 with B0 <= samples <= 16 * B0.
+ * With latency D, b200conv_process writes out[c][i] = y[c][n0 + i - D], y = what the same handle returns at zero
+ * latency fed head-block calls, n0 = the call's first absolute sample; samples before 0 are exact zeros.  Any call
+ * length and the routing work as usual.  b200conv_chain_process delays the whole mix the same way (dry and wet stay
+ * aligned); b200conv_chain_update takes effect at the next head-block step; b200conv_chain_swap needs equal latencies
+ * on both handles (else B200CONV_EINVAL) and counts its warm-up and fade in head-block steps.
+ * The call only copies the samples into a pinned ring, enqueues one step per head block the samples complete (one
+ * launch on the real-time shapes) and copies out the output of blocks earlier calls completed: it waits for the device
+ * only if a needed block has not finished yet.
+ * Call after the IR is loaded; it clears the handle (b200conv_clear).  init_* and b200conv_reset return the handle to
+ * zero latency.  b200conv_clear waits for the enqueued steps; the next D samples are zeros again.
+ * B200CONV_EINVAL: not a multiple / out of range.  B200CONV_ESTATE: no IR, a sharded handle, an attached slot exchange,
+ * a pending IR hot swap.  On a latency handle b200conv_process_device*, b200conv_process_sliced*, b200conv_prime and
+ * b200conv_process_xfade fail with B200CONV_ESTATE.  A latency handle is driven through either b200conv_process or
+ * b200conv_chain_process, not both. */
+int    b200conv_set_latency(b200conv_t* h, size_t samples);
+size_t b200conv_latency(const b200conv_t* h);
+/* calls in fixed-latency mode that had to wait for device work (the host's underrun indicator); reset by set_latency */
+unsigned long long b200conv_latency_waits(const b200conv_t* h);
+
 /* Introspection --------------------------------------------------------------------------- */
 typedef struct b200conv_stage_info {
   size_t block;        /* B_s                                  */

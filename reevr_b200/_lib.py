@@ -76,6 +76,9 @@ SYMBOLS = [
     ("b200conv_process_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int]),
     ("b200conv_clear", C.c_int, [C.c_void_p]),
     ("b200conv_reset", C.c_int, [C.c_void_p]),
+    ("b200conv_set_latency", C.c_int, [C.c_void_p, C.c_size_t]),
+    ("b200conv_latency", C.c_size_t, [C.c_void_p]),
+    ("b200conv_latency_waits", C.c_ulonglong, [C.c_void_p]),
     ("b200conv_num_stages", C.c_int, [C.c_void_p]),
     ("b200conv_stage", C.c_int, [C.c_void_p, C.c_int, C.POINTER(StageInfo)]),
     ("b200conv_ir_len", C.c_size_t, [C.c_void_p, C.c_int]),

@@ -229,6 +229,20 @@ class Engine:
     def reset(self):
         self._check(self._l.b200conv_reset(self._h), "reset")
 
+    def set_latency(self, samples: int) -> None:
+        """Fixed-latency mode (b200conv_set_latency): process / chain_process return their output `samples` later
+        (0 = zero latency, else a multiple of the head block up to 16 head blocks).  Clears the handle."""
+        self._check(self._l.b200conv_set_latency(self._h, samples), "set_latency")
+
+    @property
+    def latency(self) -> int:
+        return int(self._l.b200conv_latency(self._h))
+
+    @property
+    def latency_waits(self) -> int:
+        """Calls in fixed-latency mode that had to wait for the device (an underrun indicator)."""
+        return int(self._l.b200conv_latency_waits(self._h))
+
     # -- introspection ---------------------------------------------------------------------
     def stages(self) -> list:
         out = []

@@ -181,6 +181,10 @@ struct ChainWetParams {
   // reference's `xfade` counter at sample 0 of this launch, xfadelen its start value
   const float* conv_in;
   long long xfade0, xfadelen;
+  // fixed-latency steps: completion word in pinned host memory (nullptr: none), raised to done_val by the last CTA to
+  // finish (ticket: a device word that is 0 between launches) after every CTA's output stores
+  unsigned int* done_flag; unsigned int done_val;
+  unsigned int* ticket;
 };
 
 // * yrev ; mid/side width ; dry / wet mix of one sample of the summed wet signal (src/PluginProcessor.cpp:1840-1876)
@@ -264,14 +268,30 @@ static __global__ void __launch_bounds__(1024) k_chain_send(ChainSendParams P) {
   for (long long i = t; i < P.n; i += T) chain_ring_read(P, ch, i);
 }
 
+// the pattern of k_rt_block's done_flag across the CTAs of a grid: every thread's stores are released system-wide, the
+// CTA meets, and the CTA that draws the last ticket raises the word
+static __device__ __forceinline__ void chain_wet_done(const ChainWetParams& P) {
+  if (!P.done_flag) return;
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x == 0 && atomicAdd(P.ticket, 1u) == gridDim.x - 1) {
+    atomicExch(P.ticket, 0u);
+    __threadfence_system();
+    *reinterpret_cast<volatile unsigned int*>(P.done_flag) = P.done_val;
+    __threadfence_system();
+  }
+}
+
 static __global__ void k_chain_wet(ChainWetParams P) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < P.n) chain_wet_sample(P, i);
+  chain_wet_done(P);
 }
 
 static __global__ void k_chain_wet_xfade(ChainWetParams P) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < P.n) chain_wet_xfade_sample(P, i);
+  chain_wet_done(P);
 }
 #else
 // CPU emulation (tests/emu): same chunking, same two passes
@@ -317,9 +337,11 @@ inline void emu_chain_send(const ChainSendParams& P, int T) {
 }
 inline void emu_chain_wet(const ChainWetParams& P) {
   for (long long i = 0; i < P.n; ++i) chain_wet_sample(P, i);
+  if (P.done_flag) *P.done_flag = P.done_val;
 }
 inline void emu_chain_wet_xfade(const ChainWetParams& P) {
   for (long long i = 0; i < P.n; ++i) chain_wet_xfade_sample(P, i);
+  if (P.done_flag) *P.done_flag = P.done_val;
 }
 #endif
 

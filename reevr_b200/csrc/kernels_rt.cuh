@@ -454,4 +454,17 @@ inline void emu_rt_block(const RtParams& P) {
 }
 #endif
 
+// Completion word of a fixed-latency step that ran as several launches and copies (b200conv_set_latency): one thread,
+// queued behind the step's last operation on the same stream, makes everything before it visible system-wide and
+// raises the sequence value.
+#if defined(__CUDACC__)
+static __global__ void k_seq_flag(unsigned int* flag, unsigned int val) {
+  __threadfence_system();
+  *reinterpret_cast<volatile unsigned int*>(flag) = val;
+  __threadfence_system();
+}
+#else
+inline void emu_seq_flag(unsigned int* flag, unsigned int val) { *flag = val; }
+#endif
+
 }  // namespace pc
