@@ -68,11 +68,17 @@ int b200conv_init_stages(b200conv_t* h, int n_stages, const size_t* blocks, cons
  * TwoStageFFTConvolver::process TwoStageFFTConvolver.cpp:151-233): in[c] / out[c] are HOST
  * pointers to `len` float32 samples per channel; any len >= 0, zero added latency, output is
  * complete on return.  in/out may not alias (same rule as the reference, SURVEY §8a-2).
+ * A call of at most one head block (len <= head block size, whether or not it crosses a head-block
+ * boundary, so any host block size a REEV-R host uses) is one cluster-kernel launch with zero-copy
+ * I/O, plus the tail blocks it completes, on handles whose later stages' blocks are multiples of the
+ * head block; uniform handles whose head stage is too large for one cluster run such a call as
+ * three launches if it stays inside the open block and on the multi-kernel path if it crosses.
  * Long calls are internally cut into block batches and pipelined over PCIe. */
 int b200conv_process(b200conv_t* h, const float* const* in, float* const* out, size_t len);
 
 /* Same, with DEVICE-resident buffers: channel c at in_dev + c*in_stride (floats).  Asynchronous
- * on the handle's stream unless sync != 0.  This is the throughput path bench.py times. */
+ * on the handle's stream unless sync != 0.  This is the throughput path bench.py times; a call of
+ * at most one head block takes the same one-launch path as b200conv_process. */
 int b200conv_process_device(b200conv_t* h, const float* in_dev, size_t in_stride,
                             float* out_dev, size_t out_stride, size_t len, int sync);
 
@@ -137,8 +143,8 @@ unsigned long long b200conv_launch_count(const b200conv_t* h);
 /* Form of the FDL sweep (FFTConvolver.cpp:176-187) the last launch resolved to: 22 / 26 = packed-FMA batched sweep,
  * 40 = tensor-core sweep (wgmma f16, 3xFP16 with power-of-two scales), 100..108 = streaming forms.  For benchmarks and tests. */
 int b200conv_last_sweep_variant(const b200conv_t* h);
-/* Tuning / A-B switches: "rt" (1 = real-time calls that stay inside the open block run as ONE cluster-kernel launch
- * with zero-copy I/O, 0 = multi-kernel path), "fft512" (1 = register-resident FFT kernels for block size 512),
+/* Tuning / A-B switches: "rt" (1 = real-time calls of at most one head block run as ONE cluster-kernel launch
+ * with zero-copy I/O, see b200conv_process; 0 = multi-kernel path), "fft512" (1 = register-resident FFT kernels for block size 512),
  * "slice_keep_tail" (default 1; 0 = b200conv_process_sliced does not upload / transform the last P blocks of the call:
  * the handle then only supports a following sliced call whose slice starts >= P blocks into the call — every rank
  * but 0 of a steady batch job — until the next b200conv_clear), "stream_alternate" (default 1: the streaming sweep

@@ -1992,8 +1992,17 @@ int rt_cluster_ctas(const b200conv* h, size_t len) {
   if (!whole_head || h->p2p_on || h->timing || h->yprev_stale) return 0;
   const Stage& s0 = h->stages[0];
   const int M = s0.B, C = h->C;
-  if (M < 16 || M > 1024 || C > 8 || len == 0 || (size_t)s0.fill + len > (size_t)M) return 0;
+  if (M < 16 || M > 1024 || C > 8 || len == 0 || len > (size_t)M) return 0;
   if (h->route_on && (h->n_out * (int)len > 8 * 1024)) return 0;
+  // A call that completes the open block and starts the next one runs as two segments.  Every later stage's block must
+  // then end on head-block boundaries only, and a stage whose block completes at this boundary must not be needed
+  // before the call ends: its block is enqueued after the launch, and with q = 1 its output starts at the boundary.
+  const bool cross = (size_t)s0.fill + len > (size_t)M;
+  if (cross)
+    for (size_t si = 1; si < h->stages.size(); ++si) {
+      const Stage& s = h->stages[si];
+      if (s.B % M != 0 || (s.q < 2 && s.fill + (M - s0.fill) == s.B)) return 0;
+    }
   int max_nc = 1;
   while (max_nc * 2 * C <= 16 && max_nc * 2 <= M / 32) max_nc *= 2;     // cluster <= 16 CTAs, tile >= 16 bin pairs
   int nc = 1;
@@ -2002,8 +2011,8 @@ int rt_cluster_ctas(const b200conv* h, size_t len) {
   // one SM pulls ~20-50 GB/s out of L2 with this access pattern: spread a convolver over as many CTAs as the
   // cluster allows until a CTA streams <= 64 KB; beyond kRtMaxBytesPerCta the all-SM streaming sweep wins
   while (nc < max_nc && bytes / nc > 64 * 1024) nc *= 2;
-  if (nc > max_nc || bytes / nc > kRtMaxBytesPerCta)
-    return (C <= 8 && M >= 64) ? -1 : 0;        // -1: split mode (front kernel, all-SM TMA sweep, back kernel)
+  if (nc > max_nc || bytes / nc > kRtMaxBytesPerCta)      // -1: split mode (front kernel, all-SM TMA sweep, back
+    return (!cross && C <= 8 && M >= 64) ? -1 : 0;        // kernel) for calls inside the open block
   return nc;
 }
 
@@ -2046,26 +2055,47 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
         h->rt_tail_joined = true;
       }
   }
-  if (int rc = ensure_rows(h, s0, 1)) return rc;
+  // a call that crosses the block boundary: len1 samples complete the open block, the other r start the next one
+  const int len1 = std::min((int)len, M - s0.fill), r = (int)len - len1;
+  if (int rc = ensure_rows(h, s0, r ? 2 : 1)) return rc;
   pc::RtParams P{};
   P.M = M; P.C = C; P.NC = nc; P.P = s0.P;
-  P.fill = s0.fill; P.len = (int)len; P.complete = (s0.fill + (int)len == M) ? 1 : 0;
+  P.len = (int)len; P.nseg = r ? 2 : 1;
+  pc::RtSeg& S1 = P.seg[0];
+  pc::RtSeg& S2 = P.seg[1];
+  S1.fill = s0.fill; S1.len = len1; S1.complete = (s0.fill + len1 == M) ? 1 : 0; S1.off = 0;
+  S1.head = s0.head; S1.abs0 = h->abs_pos - s0.fill;
+  S2.fill = 0; S2.len = r; S2.complete = 0; S2.off = len1;
+  S2.head = s0.head + 1; S2.abs0 = h->abs_pos + len1;
   P.in = in; P.in_stride = (long long)in_stride;
   for (int c = 0; c < 8; ++c) P.in_map[c] = (h->route_on || h->route_in_only) ? h->in_map[c] : c;
   P.inbuf0 = s0.inbuf; P.inbuf0_stride = (long long)s0.in_stride;
   P.H = s0.H; P.h_cstride = (long long)s0.Prows * M;
-  P.X = s0.X; P.x_cstride = (long long)s0.R * M; P.head = s0.head;
+  P.X = s0.X; P.x_cstride = (long long)s0.R * M;
   P.Yprev = s0.Y[s0.ybuf]; P.Ynext = s0.Y[s0.ybuf ^ 1]; P.y_cstride = M;
   P.tw = s0.tw;
   int na = 0;
   for (size_t si = 1; si < h->stages.size(); ++si) {
     Stage& s = h->stages[si];
-    P.later_inbuf[na] = s.inbuf; P.later_stride[na] = (long long)s.in_stride; P.later_fill[na] = s.fill;
+    P.later_stride[na] = (long long)s.in_stride;
+    S1.later_inbuf[na] = s.inbuf; S1.later_fill[na] = s.fill;
+    // a stage whose block completes at the boundary takes the samples after it at the front of its other buffer
+    const bool at_boundary = r && s.fill + len1 == s.B;
+    S2.later_inbuf[na] = at_boundary ? s.inbuf_alt : s.inbuf; S2.later_fill[na] = at_boundary ? 0 : s.fill + len1;
+    // That buffer was read by the stage's previous tail block on s_tail, so s_main must be ordered behind it.  With
+    // q <= 2 (every two-stage handle) the loop above has already waited for it, as it does for the first call after the
+    // buffer swap below: that block's output starts at (blocks_done - 1 + q) * B, at or before the boundary, and this
+    // call ends after the boundary.  Deeper stages of b200conv_init_stages wait here.
+    const int jp = (int)((s.njobs + 1) & 1);
+    if (at_boundary && s.njobs && !s.job_waited[jp]) {
+      CU_CHECK(h, cudaStreamWaitEvent(h->s_main, s.ev_job[jp], 0));
+      s.job_waited[jp] = true;
+      h->rt_tail_joined = true;
+    }
     P.add[na] = s.fut; P.add_cstride[na] = (long long)s.ring; P.add_mask[na] = (long long)s.ring - 1;
     ++na;
   }
   P.n_later = na; P.n_add = na;
-  P.abs0 = h->abs_pos - s0.fill;
   P.out = out; P.out_stride = (long long)out_stride;
   P.mix_on = h->route_on ? 1 : 0; P.n_out = h->route_on ? h->n_out : C;
   std::memcpy(P.mix, h->mix, sizeof(P.mix));
@@ -2109,15 +2139,15 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
     if (int rc = launch(P)) return rc;
   }
   // bookkeeping of the head stage
-  if (P.complete) { s0.head += 1; s0.blocks_done += 1; s0.fill = 0; s0.ybuf ^= 1; }
+  if (S1.complete) { s0.head += 1; s0.blocks_done += 1; s0.fill = r; s0.ybuf ^= 1; }
   else s0.fill += (int)len;
   h->abs_pos += (long long)len;
   // later stages: the kernel appended the samples; a completed block goes to the low-priority stream
   bool recorded = false;
   for (size_t si = 1; si < h->stages.size(); ++si) {
     Stage& s = h->stages[si];
-    s.fill += (int)len;
-    if (s.fill < s.B) continue;
+    s.fill += len1;
+    if (s.fill < s.B) { s.fill += r; continue; }
     if (!recorded) { CU_CHECK(h, cudaEventRecord(h->ev_rt, h->s_main)); recorded = true; }
     CU_CHECK(h, cudaStreamWaitEvent(h->s_tail, h->ev_rt, 0));
     const int j = (int)(s.njobs & 1);
@@ -2130,6 +2160,7 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
     s.job_waited[j] = false;
     s.njobs++;
     std::swap(s.inbuf, s.inbuf_alt);              // the following calls fill the other buffer
+    s.fill = r;                                   // ... which holds the samples after the boundary
   }
   return 0;
 }
@@ -2377,7 +2408,7 @@ int b200conv_process_device(b200conv_t* h, const float* in_dev, size_t in_stride
     const size_t chunk = h->Lmax - B0;     // keeps fill + n <= Lmax for every stage (inbuf holds B + Lmax samples)
     const bool overlap = len > chunk || h->cfg.shard_count > 1;    // (slot-exchange groups always use s_post)
     size_t done = 0;
-    if (const int nc = rt_cluster_ctas(h, len)) {       // a call inside the open block: one cluster kernel
+    if (const int nc = rt_cluster_ctas(h, len)) {       // a call of at most one head block: one cluster kernel
       if (int rc = rt_call(h, nc, in_dev, in_stride, out_dev, out_stride, len, nullptr, 0)) return rc;
       done = len;
     }
