@@ -225,6 +225,23 @@ int b200conv_chain_update(b200conv_t* h, const b200conv_chain_config* cfg);
 int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* ysend, const float* yrev,
                            float* const* out, size_t len);
 
+/* The same chain on DEVICE-resident buffers, for batch work from device memory (a PyTorch pipeline, an offline render):
+ * dry L at dry_dev, R at dry_dev + dry_stride; the mix at out_dev / out_dev + out_stride (floats); ysend_dev / yrev_dev
+ * one row each (NULL = 1).  out_dev == dry_dev with out_stride == dry_stride runs in place; any other overlap is
+ * undefined.  Asynchronous on b200conv_stream(h) unless sync != 0, like b200conv_process_device: no staging copy and no
+ * synchronise between the pieces (at most Lmax - B0 samples each) the call is cut into.
+ * Semantics are b200conv_chain_process's for the same samples and call lengths, and the two entries can be mixed on one
+ * handle: b200conv_chain_update takes effect at the next call; a pending b200conv_chain_swap warms up in the first call,
+ * fades, and hands the chain over at the end of the completing call, after which the incoming handle's stream is ordered
+ * behind this call's work.
+ * Pieces shorter than 16 384 samples run the send filters exactly as b200conv_chain_process does, so a call made of such
+ * pieces is bit for bit the host call.  Longer pieces run the send filters as a chunked scan spread over the whole GPU
+ * (same FP32 chunk arithmetic, FP64 scan, different chunking): within float rounding of the host call, not bit-identical.
+ * B200CONV_ESTATE: no chain, or a fixed-latency handle.  B200CONV_EINVAL: dry_dev or out_dev NULL.  len == 0 does
+ * nothing. */
+int b200conv_chain_process_device(b200conv_t* h, const float* dry_dev, size_t dry_stride, const float* ysend_dev,
+                                  const float* yrev_dev, float* out_dev, size_t out_stride, size_t len, int sync);
+
 /* IR hot-swap inside the device chain (src/PluginProcessor.cpp:1655-1668, 1694-1756, 1799-1830).
  * `live` has the chain configured; `incoming` holds the new IR (e.g. b200conv_init_twostage_recalc).
  * The next b200conv_chain_process(live, ...) does the warm-up (0.25 s of send history, replayed on the device in

@@ -106,6 +106,8 @@ SYMBOLS = [
     ("b200conv_unregister_host", C.c_int, [C.c_void_p]),
     ("b200conv_chain_configure", C.c_int, [C.c_void_p, C.c_void_p]),
     ("b200conv_chain_process", C.c_int, [C.c_void_p, _PP, C.c_void_p, C.c_void_p, _PP, C.c_size_t]),
+    ("b200conv_chain_process_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_size_t, C.c_size_t, C.c_int]),
     ("b200conv_chain_update", C.c_int, [C.c_void_p, C.c_void_p]),
     ("b200conv_chain_swap", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     ("b200conv_chain_swap_state", C.c_int, [C.c_void_p]),

@@ -213,6 +213,14 @@ class Engine:
                 env[1].ctypes.data if env[1] is not None else None, _ptr_array(ys), n), "chain_process")
         return ys[0], ys[1]
 
+    def chain_process_device(self, dry_ptr: int, dry_stride: int, out_ptr: int, out_stride: int, n: int,
+                             ysend_ptr: int = 0, yrev_ptr: int = 0, sync: bool = False):
+        """chain_process on device buffers (b200conv_chain_process_device): dry L / R rows dry_stride floats apart, the
+        mix into out L / R rows out_stride apart (out_ptr == dry_ptr with equal strides: in place); envelope pointers 0
+        mean 1.  Asynchronous on the handle's stream unless sync."""
+        self._check(self._l.b200conv_chain_process_device(self._h, dry_ptr, dry_stride, ysend_ptr or None, yrev_ptr or None,
+                                                          out_ptr, out_stride, n, int(sync)), "chain_process_device")
+
     def chain_swap(self, incoming: "Engine", host_block: int) -> None:
         """IR hot swap inside the chain (b200conv_chain_swap): the next chain_process call replays the send history
         through `incoming` and starts the 50 ms crossfade; when chain_swap_state() becomes 3 the chain has moved to

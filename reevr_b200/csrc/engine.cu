@@ -175,6 +175,7 @@ struct b200conv {
   float* c_filt = nullptr;           // [3][Lmax]: filtered send of the call ; row 2 stays zero (LR / RL input of a
                                      // quad handle being crossfaded in)
   float* c_state = nullptr;          // [4][kChainStateStride] filter states: rows 0-1 the send, rows 2-3 the warm-up replay of a swap
+  void* c_wide = nullptr;            // scratch of the whole-GPU send form (pc::ChainWideScratch), sized for Lmax
   bool c_six[2] = {false, false};    // slot 0 of the low / high cut's state holds the 6 dB `state` (else ic1)
   float* c_hpin = nullptr;           // pinned [dry L, dry R, ysend, yrev, out L, out R][hpin_cap]: zero-copy I/O of real-time chain calls
   float* c_hpin_dev = nullptr;
@@ -377,6 +378,7 @@ void free_all(b200conv* h) {
   if (h->tc_err) cudaFreeHost(h->tc_err);
   h->tc_err = h->tc_err_dev = nullptr; h->tc_alloc_failed = false;
   cudaFree(h->c_io); cudaFree(h->c_conv_in); cudaFree(h->c_filt); cudaFree(h->c_state); cudaFree(h->c_ring);
+  cudaFree(h->c_wide); h->c_wide = nullptr;
   if (h->c_hpin) cudaFreeHost(h->c_hpin);
   h->c_hpin = h->c_hpin_dev = nullptr;
   h->c_io = h->c_conv_in = h->c_filt = h->c_state = h->c_ring = nullptr;
@@ -2947,6 +2949,50 @@ int launch_chain_send(b200conv* h, const pc::ChainSendParams& sp, cudaStream_t s
   return 0;
 }
 
+// Device-pointer pieces of at least this many samples run the whole-GPU send form (kernels_chain.cuh
+// k_chain_wide_*), shorter ones k_chain_send exactly as the host entry does.  See DESIGN §4 for the measurement.
+constexpr size_t kChainWideMin = 16384;
+
+// the whole-GPU form's scratch inside one allocation of chain_wide_bytes(Lmax): P_j, aggregates, carries, Z_c
+size_t chain_wide_bytes(size_t Lmax) {
+  const size_t nb = (size_t)pc::chain_wide_ctas((long long)Lmax), S = pc::kChainStates;
+  return (pc::kWidePowers * S * S + 4 * nb * S) * sizeof(double) + 2 * nb * pc::kWideT * S * sizeof(float);
+}
+pc::ChainWideScratch chain_wide_scratch(const b200conv* h) {
+  pc::ChainWideScratch w{};
+  const long long nb = pc::chain_wide_ctas((long long)h->Lmax), S = pc::kChainStates;
+  w.nb_cap = nb;
+  w.pw = static_cast<double*>(h->c_wide);
+  w.agg = w.pw + pc::kWidePowers * S * S;
+  w.carry = w.agg + 2 * nb * S;
+  w.z = reinterpret_cast<float*>(w.carry + 2 * nb * S);
+  return w;
+}
+
+// the whole-GPU send form of one piece; `powers`: the call's first such piece (P_j follow the filters, which change
+// only between calls)
+int launch_chain_wide(b200conv* h, const pc::ChainSendParams& sp, bool powers, cudaStream_t st) {
+  const pc::ChainWideScratch w = chain_wide_scratch(h);
+#if defined(PC_EMULATE)
+  (void)st;
+  pc::emu_chain_wide(sp, w, powers);
+  h->launches += (sp.lc.on || sp.hc.on) ? 3 + (powers ? 1 : 0) : 1;
+#else
+  const long long nb = pc::chain_wide_ctas(sp.n);
+  const dim3 grid((unsigned)nb, 2);
+  if (sp.lc.on || sp.hc.on) {
+    if (powers) { pc::k_chain_wide_powers<<<1, 64, 0, st>>>(sp, w.pw); h->launches++; }
+    pc::k_chain_wide_pass1<<<grid, pc::kWideT, 0, st>>>(sp, w);
+    pc::k_chain_wide_carry<<<2, pc::kWideCarryT, 0, st>>>(sp, w, nb);
+    h->launches += 2;
+  }
+  pc::k_chain_wide_pass2<<<grid, pc::kWideT, 0, st>>>(sp, w);
+  CU_CHECK(h, cudaGetLastError());
+  h->launches++;
+#endif
+  return 0;
+}
+
 // Filter::init (src/dsp/Filter.cpp:3-21) with the q the processor passes (src/PluginProcessor.cpp:845-848)
 pc::ChainFilter chain_filter(bool on, int slope, int mode, float srate, float freq) {
   pc::ChainFilter f{};
@@ -3048,6 +3094,7 @@ int b200conv_chain_configure(b200conv_t* h, const b200conv_chain_config* cfg) {
     CU_CHECK(h, cudaMalloc(&h->c_filt, 3 * L * sizeof(float)));
     CU_CHECK(h, cudaMemsetAsync(h->c_filt + 2 * L, 0, L * sizeof(float), h->s_main));
     CU_CHECK(h, cudaMalloc(&h->c_state, 4 * pc::kChainStateStride * sizeof(float)));
+    CU_CHECK(h, cudaMalloc(&h->c_wide, chain_wide_bytes(L)));
     CU_CHECK(h, cudaMallocHost((void**)&h->c_hpin, 6 * h->hpin_cap * sizeof(float)));
 #if defined(PC_EMULATE)
     h->c_hpin_dev = h->c_hpin;
@@ -3136,7 +3183,7 @@ int chain_warm_up(b200conv* h, b200conv* g) {
 // end of the fade: the chain (filter states, predelay / warmer ring, configuration, staging) moves to g by pointer
 void chain_move(b200conv* h, b200conv* g) {
   std::swap(h->c_io, g->c_io); std::swap(h->c_conv_in, g->c_conv_in); std::swap(h->c_filt, g->c_filt);
-  std::swap(h->c_state, g->c_state); std::swap(h->c_hpin, g->c_hpin); std::swap(h->c_hpin_dev, g->c_hpin_dev);
+  std::swap(h->c_state, g->c_state); std::swap(h->c_wide, g->c_wide); std::swap(h->c_hpin, g->c_hpin); std::swap(h->c_hpin_dev, g->c_hpin_dev);
   std::swap(h->c_ring, g->c_ring); std::swap(h->c_ring_size, g->c_ring_size); std::swap(h->c_ring_pos, g->c_ring_pos);
   std::swap(h->c_delay_len, g->c_delay_len); std::swap(h->c_delay_floor, g->c_delay_floor);
   std::swap(h->c_six[0], g->c_six[0]); std::swap(h->c_six[1], g->c_six[1]);
@@ -3151,16 +3198,19 @@ void chain_move(b200conv* h, b200conv* g) {
 
 // One piece of n samples of a chain call on h, the chain's owner, queued on the handles' streams: the send kernel, the
 // warm-up and this piece's send through the incoming handle of a pending swap, the convolvers and the wet kernel.
-// d_dry, d_send, d_rev, d_out: device addresses, rows dstride apart (d_send / d_rev nullptr: envelope 1).  `completing`:
-// the fade completes in this call (the wet kernel drops the LR / RL terms).  done_flag (fixed-latency steps): the wet
-// kernel raises it to done_val after its last store (ticket: its last-CTA counter).
-int chain_piece(b200conv* h, const float* d_dry, const float* d_send, const float* d_rev, float* d_out, size_t dstride,
-                size_t n, bool completing, unsigned int* done_flag, unsigned int done_val, unsigned int* ticket) {
+// d_dry, d_send, d_rev, d_out: device addresses, dry rows dry_stride apart and out rows out_stride apart (d_send / d_rev
+// nullptr: envelope 1).  `completing`: the fade completes in this call (the wet kernel drops the LR / RL terms).
+// done_flag (fixed-latency steps): the wet kernel raises it to done_val after its last store (ticket: its last-CTA
+// counter).  *wide_powers != nullptr: the send runs the whole-GPU form (k_chain_wide_*), which builds its matrix powers
+// when *wide_powers is set and clears it.
+int chain_piece(b200conv* h, const float* d_dry, const float* d_send, const float* d_rev, float* d_out, size_t dry_stride,
+                size_t out_stride, size_t n, bool completing, unsigned int* done_flag, unsigned int done_val,
+                unsigned int* ticket, bool* wide_powers = nullptr) {
   const int C = h->C;
   const size_t L = h->Lmax;
   b200conv* g = h->swap_live ? h->swap_peer : nullptr;
   pc::ChainSendParams sp{};
-  sp.dry = d_dry; sp.dry_stride = (long long)dstride; sp.ysend = d_send;
+  sp.dry = d_dry; sp.dry_stride = (long long)dry_stride; sp.ysend = d_send;
   sp.conv_in = h->c_conv_in; sp.conv_stride = (long long)L;
   sp.filt = h->c_filt; sp.filt_stride = (long long)L;
   sp.state = h->c_state;
@@ -3173,7 +3223,13 @@ int chain_piece(b200conv* h, const float* d_dry, const float* d_send, const floa
     sp.swap_lc = h->c_six[0] != (sp.lc.slope == 0); sp.swap_hc = h->c_six[1] != (sp.hc.slope == 0);
     h->c_six[0] = sp.lc.slope == 0; h->c_six[1] = sp.hc.slope == 0;
   }
-  if (int rc = launch_chain_send(h, sp, h->s_main)) return rc;
+  if (wide_powers) {
+    if (!g) sp.filt = nullptr;          // only the incoming convolver of a fading swap reads the undelayed send
+    if (int rc = launch_chain_wide(h, sp, *wide_powers, h->s_main)) return rc;
+    if (sp.lc.on || sp.hc.on) *wide_powers = false;
+  } else if (int rc = launch_chain_send(h, sp, h->s_main)) {
+    return rc;
+  }
   h->c_ring_pos += (long long)n;
   if (g) {
     // the incoming handle runs on its own stream behind the send kernel: warm-up (first piece), then this piece's
@@ -3190,10 +3246,10 @@ int chain_piece(b200conv* h, const float* d_dry, const float* d_send, const floa
   // the convolvers: LL, RR[, LR, RL] read the chain's L / R, per-convolver outputs stay on the device
   if (int rc = chain_convolve(h, h->c_conv_in, L, n)) return rc;
   pc::ChainWetParams wp{};
-  wp.dry = d_dry; wp.dry_stride = (long long)dstride;
+  wp.dry = d_dry; wp.dry_stride = (long long)dry_stride;
   wp.conv = h->dch[0]; wp.conv_stride = (long long)L;
   wp.yrev = d_rev;
-  wp.out = d_out; wp.out_stride = (long long)dstride; wp.n = (long long)n;
+  wp.out = d_out; wp.out_stride = (long long)out_stride; wp.n = (long long)n;
   wp.quad_ts = (C == 4 && h->chain_cfg.true_stereo) ? 1 : 0;
   wp.width = h->chain_cfg.width; wp.drygain = h->chain_cfg.drygain; wp.wetgain = h->chain_cfg.wetgain;
   wp.done_flag = done_flag; wp.done_val = done_val; wp.ticket = ticket;
@@ -3234,7 +3290,7 @@ static int chain_process_latency(b200conv_t* h, const float* const* dry, const f
     b200conv* g = x->swap_live ? x->swap_peer : nullptr;
     const bool completing = g && x->swap_xfade - (long long)B <= 0;
     r->last_st = x->s_main;
-    if (int rc = chain_piece(x, d, d + 2 * L, d + 3 * L, r->out_dev + off, L, B, completing, r->word_dev, v, r->ticket))
+    if (int rc = chain_piece(x, d, d + 2 * L, d + 3 * L, r->out_dev + off, L, L, B, completing, r->word_dev, v, r->ticket))
       return rc;
     if (g && x->swap_xfade <= 0) {                  // src/PluginProcessor.cpp:1823-1826
       chain_move(x, g);
@@ -3284,8 +3340,8 @@ int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* 
       if (ysend) CU_CHECK(h, cudaMemcpyAsync(d_send, ysend + done, n * sizeof(float), cudaMemcpyHostToDevice, h->s_main));
       if (yrev) CU_CHECK(h, cudaMemcpyAsync(d_rev, yrev + done, n * sizeof(float), cudaMemcpyHostToDevice, h->s_main));
     }
-    if (int rc = chain_piece(h, d_dry, ysend ? d_send : nullptr, yrev ? d_rev : nullptr, d_out, dstride, n, completing,
-                             nullptr, 0, nullptr)) return rc;
+    if (int rc = chain_piece(h, d_dry, ysend ? d_send : nullptr, yrev ? d_rev : nullptr, d_out, dstride, dstride, n,
+                             completing, nullptr, 0, nullptr)) return rc;
     if (!zc)
       for (int ch = 0; ch < 2; ++ch)
         CU_CHECK(h, cudaMemcpyAsync(out[ch] + done, d_out + ch * L, n * sizeof(float), cudaMemcpyDeviceToHost, h->s_main));
@@ -3295,6 +3351,38 @@ int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* 
     done += n;
   }
   if (g && h->swap_xfade <= 0) chain_move(h, g);        // src/PluginProcessor.cpp:1823-1826
+  return B200CONV_OK;
+}
+
+// The chain on the caller's device buffers: the pieces of b200conv_chain_process without staging copies or a
+// synchronise between them.  Pieces of at least kChainWideMin samples run the whole-GPU send form.
+int b200conv_chain_process_device(b200conv_t* h, const float* dry_dev, size_t dry_stride, const float* ysend_dev,
+                                  const float* yrev_dev, float* out_dev, size_t out_stride, size_t len, int sync) {
+  REQUIRE_CUDA(h);
+  if (len == 0) return B200CONV_OK;
+  if (!h->chain_on) return fail(h, B200CONV_ESTATE, "b200conv_chain_configure first");
+  if (h->lat_D) return fail(h, B200CONV_ESTATE, "device-pointer calls are not available in fixed-latency mode");
+  if (!dry_dev || !out_dev) return fail(h, B200CONV_EINVAL, "null buffer");
+  if (h->stages.empty()) return fail(h, B200CONV_ESTATE, "no impulse response loaded");
+  if (int rc = set_device(h)) return rc;
+  const size_t L = h->Lmax, B0 = h->stages[0].B;
+  b200conv* g = h->swap_live ? h->swap_peer : nullptr;
+  const size_t chunk = g ? std::min(L - B0, L - (size_t)g->stages[0].B) : L - B0;
+  const bool completing = g && h->swap_xfade - (long long)len <= 0;
+  bool powers = true;
+  for (size_t done = 0; done < len;) {
+    const size_t n = std::min(len - done, chunk);
+    if (int rc = chain_piece(h, dry_dev + done, ysend_dev ? ysend_dev + done : nullptr, yrev_dev ? yrev_dev + done : nullptr,
+                             out_dev + done, dry_stride, out_stride, n, completing, nullptr, 0, nullptr,
+                             n >= kChainWideMin ? &powers : nullptr)) return rc;
+    done += n;
+  }
+  if (g && h->swap_xfade <= 0) {        // the chain moves to g; g's next call runs behind this one
+    chain_move(h, g);
+    CU_CHECK(h, cudaEventRecord(h->ev_h2d[0], h->s_main));
+    CU_CHECK(g, cudaStreamWaitEvent(g->s_main, h->ev_h2d[0], 0));
+  }
+  if (sync) CU_CHECK(h, cudaStreamSynchronize(h->s_main));
   return B200CONV_OK;
 }
 

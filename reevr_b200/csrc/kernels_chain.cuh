@@ -218,6 +218,95 @@ PC_HD void chain_wet_xfade_sample(const ChainWetParams& P, long long i) {
   chain_wet_mix(P, i, wl, wr);
 }
 
+// ---- the whole-GPU send form of long device-pointer pieces (b200conv_chain_process_device) -------------------------
+// The math of k_chain_send, spread over as many CTAs as the piece needs, both channels in one grid: chunks of a fixed
+// kWideLc samples, one per thread, kWideT chunks per CTA.  Four launches:
+//   powers  k_chain_wide_powers: A from one zero-input step (chain_power_column), squared in double to
+//           P_j = A^(kWideLc * 2^j), j < kWidePowers (once per call: the filters do not change within a call)
+//   pass 1  k_chain_wide_pass1: every chunk from a zero state gives its end state Z_c (FP32, as chain_run_chunk runs
+//           it); the CTA folds its Z_c in double into its aggregate sum_c M^(last - c) Z_c (M = P_0 = A^Lc) by a tree
+//   carry   k_chain_wide_carry: one CTA per channel scans the aggregates, G_{b+1} = M^kWideT G_b + agg_b from
+//           G_0 = chain_scan_start (the stash exchange and the carried state as in k_chain_send), Hillis-Steele in
+//           tiles of kWideCarryT with P_{log2 kWideT + j} as the multipliers
+//   pass 2  k_chain_wide_pass2: the CTA scans its Z_c again, seeded with G_b, for every chunk's true initial state
+//           (rounded to float), re-runs the chunks and writes the ring and the predelayed convolver input
+// Only the last chunk of a piece can be ragged; nothing downstream of it is read, so no chunk advances by less than M.
+// The send is staged through shared memory (row per chunk, padded against bank conflicts), so every global access is
+// coalesced.  Pass 2 needs no grid barrier for the predelay: conv_in[i] for i >= predelay is the pass-2 value of sample
+// i - predelay, written by whichever thread owns that sample; conv_in[i] for i < predelay reads a ring slot of an
+// earlier piece, at a distance of at most predelay + n - 1 < ring size (chain_ring_len: >= D + Lmax + 1, predelay <=
+// D, n <= Lmax) from every slot this piece writes.  Deterministic: fixed chunking, fixed reduction and scan order.
+constexpr int kWideLc = 64;                // samples per chunk
+constexpr int kWideT = 128;                // chunks (threads) per CTA
+constexpr int kWideSpan = kWideLc * kWideT;
+constexpr int kWideLogT = 7;
+constexpr int kWideCarryT = 512;           // threads of the carry scan: a tile carries 511 aggregates
+constexpr int kWideLogCarry = 9;
+constexpr int kWideLogLc = 6;
+constexpr int kWidePowers = kWideLogT + kWideLogCarry;
+
+// scratch of the whole-GPU form, sized for Lmax (b200conv_chain_configure)
+struct ChainWideScratch {
+  double* pw;                              // [kWidePowers][8][8] P_j
+  double* agg;                             // [2][nb_cap][8] CTA aggregates
+  double* carry;                           // [2][nb_cap][8] G_b: the state entering CTA b
+  float* z;                                // [2][nb_cap * kWideT][8] zero-state end points
+  long long nb_cap;
+};
+
+inline long long chain_wide_ctas(long long n) { return (n + kWideSpan - 1) / kWideSpan; }
+
+// entry (q, r) of M * M
+PC_HD double chain_square_entry(const double (*M)[kChainStates], int q, int r) {
+  double a = 0.0;
+#pragma unroll
+  for (int k = 0; k < kChainStates; ++k) a = fma(M[q][k], M[k][r], a);
+  return a;
+}
+
+// acc += M x.  M is not read through a volatile pointer (unlike chain_scan_step's A^L): every scan step uses another
+// power, so there is nothing to hoist, and volatile loads would serialise the 64 shared-memory reads of each step
+PC_HD void chain_affine_acc(const double (*M)[kChainStates], const double* x, double* acc) {
+#pragma unroll
+  for (int q = 0; q < kChainStates; ++q) {
+    double a = acc[q];
+#pragma unroll
+    for (int r = 0; r < kChainStates; ++r) a = fma(M[q][r], x[r], a);
+    acc[q] = a;
+  }
+}
+
+// one combine step over a [kChainStates][N] array of double states: nx = V[t] + M V[t - d]  (t >= d), or
+// V[t] + M V[t + d] read as "left then right" when `tree` (pass 1: V[t] <- M V[t] + V[t + d])
+PC_HD void chain_combine(const double (*M)[kChainStates], const double* V, int N, int t, int d, bool tree,
+                         double* nx) {
+  double x[kChainStates];
+#pragma unroll
+  for (int q = 0; q < kChainStates; ++q) {
+    nx[q] = tree ? V[q * N + t + d] : V[q * N + t];
+    x[q] = tree ? V[q * N + t] : V[q * N + t - d];
+  }
+  chain_affine_acc(M, x, nx);
+}
+
+// the send sample i of channel ch (no replay: the whole-GPU form is never a warm-up)
+PC_HD float chain_wide_send(const ChainSendParams& P, int ch, long long i) {
+  const float v = P.dry[(long long)ch * P.dry_stride + i];
+  return P.ysend ? v * P.ysend[i] : v;
+}
+
+// pass 2's output of sample i (y): ring slot, predelayed convolver input, and the undelayed send while a swap fades
+PC_HD void chain_wide_store(const ChainSendParams& P, int ch, long long i, float y) {
+  P.ring[(long long)ch * P.ring_stride + ((P.ring_pos + i) & P.ring_mask)] = y;
+  if (i + P.predelay < P.n) P.conv_in[(long long)ch * P.conv_stride + i + P.predelay] = y;
+  if (i < P.predelay) {
+    const long long p = P.ring_pos + i - P.predelay;
+    P.conv_in[(long long)ch * P.conv_stride + i] =
+        p < P.delay_floor ? 0.0f : P.ring[(long long)ch * P.ring_stride + (p & P.ring_mask)];
+  }
+  if (P.filt) P.filt[(long long)ch * P.filt_stride + i] = y;
+}
+
 #if defined(__CUDACC__)
 // grid (2 channels), block T threads (T = 64 for real-time calls, 1024 for batches); static smem
 static __global__ void __launch_bounds__(1024) k_chain_send(ChainSendParams P) {
@@ -293,6 +382,166 @@ static __global__ void k_chain_wet_xfade(ChainWetParams P) {
   if (i < P.n) chain_wet_xfade_sample(P, i);
   chain_wet_done(P);
 }
+
+// whole-GPU send form (see above).  One CTA of 64 threads: A, then kWideLogLc + kWidePowers - 1 squarings
+static __global__ void __launch_bounds__(64) k_chain_wide_powers(ChainSendParams P, double* pw) {
+  __shared__ double M[kChainStates][kChainStates];
+  const int t = threadIdx.x, q = t / kChainStates, r = t % kChainStates;
+  if (t < kChainStates) {
+    double col[kChainStates];
+    chain_power_column(P, 1, t, col);
+#pragma unroll
+    for (int k = 0; k < kChainStates; ++k) M[k][t] = col[k];
+  }
+  __syncthreads();
+  for (int s = 1; s < kWideLogLc + kWidePowers; ++s) {      // M = A^(2^s)
+    const double a = chain_square_entry(M, q, r);
+    __syncthreads();
+    M[q][r] = a;
+    if (s >= kWideLogLc) pw[(s - kWideLogLc) * kChainStates * kChainStates + t] = a;
+    __syncthreads();
+  }
+}
+
+// the CTA's kWideSpan send samples of channel ch into shared memory, one padded row per chunk (coalesced loads)
+static __device__ __forceinline__ void chain_wide_stage(const ChainSendParams& P, int ch, long long base,
+                                                        float (*buf)[kWideLc + 1]) {
+  for (int j = threadIdx.x; j < kWideSpan; j += kWideT) {
+    const long long i = base + j;
+    buf[j / kWideLc][j % kWideLc] = i < P.n ? chain_wide_send(P, ch, i) : 0.0f;
+  }
+}
+
+// inclusive Hillis-Steele scan of V[kChainStates][N] with multipliers Mj[j] = M^(2^j): V[t] <- sum_k M^(t-k) V[k]
+template <int N>
+static __device__ __forceinline__ void chain_wide_scan(const double (*Mj)[kChainStates][kChainStates], double* V) {
+  const int t = threadIdx.x;
+#pragma unroll 1
+  for (int j = 0, d = 1; d < N; ++j, d *= 2) {
+    double nx[kChainStates];
+    if (t >= d) chain_combine(Mj[j], V, N, t, d, false, nx);
+    __syncthreads();
+    if (t >= d) {
+#pragma unroll
+      for (int q = 0; q < kChainStates; ++q) V[q * N + t] = nx[q];
+    }
+    __syncthreads();
+  }
+}
+
+// samples of chunk t (0 .. kWideLc) of the CTA starting at base
+static __device__ __forceinline__ int chain_wide_len(long long n, long long i0) {
+  return i0 >= n ? 0 : (n - i0 < kWideLc ? (int)(n - i0) : kWideLc);
+}
+
+// pass 1: zero-state end points Z_c and the CTA aggregate.  grid (CTAs, 2 channels)
+static __global__ void __launch_bounds__(kWideT) k_chain_wide_pass1(ChainSendParams P, ChainWideScratch W) {
+  __shared__ float buf[kWideT][kWideLc + 1];
+  __shared__ double V[kChainStates * kWideT];
+  __shared__ double PW[kWideLogT][kChainStates][kChainStates];
+  const int ch = blockIdx.y, b = blockIdx.x, t = threadIdx.x;
+  const long long base = (long long)b * kWideSpan;
+  chain_wide_stage(P, ch, base, buf);
+  for (int j = t; j < kWideLogT * kChainStates * kChainStates; j += kWideT) (&PW[0][0][0])[j] = W.pw[j];
+  __syncthreads();
+  float s[kChainStates];
+#pragma unroll
+  for (int q = 0; q < kChainStates; ++q) s[q] = 0.0f;
+  const int m = chain_wide_len(P.n, base + (long long)t * kWideLc);
+  for (int k = 0; k < m; ++k) (void)chain_cascade<float>(P, s, buf[t][k]);
+  float* z = W.z + (((long long)ch * W.nb_cap + b) * kWideT + t) * kChainStates;
+#pragma unroll
+  for (int q = 0; q < kChainStates; ++q) { z[q] = s[q]; V[q * kWideT + t] = s[q]; }
+  __syncthreads();
+  // tree: the segment at t (length d) absorbs the one at t + d: V[t] <- M^d V[t] + V[t + d]
+#pragma unroll 1
+  for (int j = 0, d = 1; d < kWideT; ++j, d *= 2) {
+    double nx[kChainStates];
+    const bool act = (t & (2 * d - 1)) == 0;
+    if (act) chain_combine(PW[j], V, kWideT, t, d, true, nx);
+    __syncthreads();
+    if (act) {
+#pragma unroll
+      for (int q = 0; q < kChainStates; ++q) V[q * kWideT + t] = nx[q];
+    }
+    __syncthreads();
+  }
+  if (t < kChainStates) W.agg[((long long)ch * W.nb_cap + b) * kChainStates + t] = V[t * kWideT];
+}
+
+// carry: G_0 = the scan's initial state, G_{b+1} = M^kWideT G_b + agg_b.  grid (2 channels)
+static __global__ void __launch_bounds__(kWideCarryT) k_chain_wide_carry(ChainSendParams P, ChainWideScratch W, long long nb) {
+  __shared__ double V[kChainStates * kWideCarryT];
+  __shared__ double Q[kWideLogCarry][kChainStates][kChainStates];
+  const int ch = blockIdx.x, t = threadIdx.x;
+  for (int j = t; j < kWideLogCarry * kChainStates * kChainStates; j += kWideCarryT)
+    (&Q[0][0][0])[j] = W.pw[kWideLogT * kChainStates * kChainStates + j];
+  __shared__ double c[kChainStates];      // G at the start of the tile (in shared memory: no registers across tiles)
+  if (t == 0) chain_scan_start(P, ch, c);
+  const double* agg = W.agg + (long long)ch * W.nb_cap * kChainStates;
+  double* G = W.carry + (long long)ch * W.nb_cap * kChainStates;
+  // tile: slot 0 holds G_g0, slot k > 0 agg_{g0 + k - 1}; after the scan slot k holds G_{g0 + k}
+#pragma unroll 1
+  for (long long g0 = 0; g0 < nb; g0 += kWideCarryT - 1) {
+    __syncthreads();
+    const long long a = g0 + t - 1;
+#pragma unroll
+    for (int q = 0; q < kChainStates; ++q)
+      V[q * kWideCarryT + t] = t == 0 ? c[q] : (a < nb - 1 ? agg[a * kChainStates + q] : 0.0);
+    __syncthreads();
+    chain_wide_scan<kWideCarryT>(Q, V);
+    if (g0 + t < nb) {
+#pragma unroll
+      for (int q = 0; q < kChainStates; ++q) G[(g0 + t) * kChainStates + q] = V[q * kWideCarryT + t];
+    }
+    if (t < kChainStates) c[t] = V[t * kWideCarryT + kWideCarryT - 1];
+  }
+}
+
+// pass 2: true initial states, the filtered chunks, ring + predelayed convolver input (+ the undelayed send while a
+// swap fades).  grid (CTAs, 2 channels)
+static __global__ void __launch_bounds__(kWideT) k_chain_wide_pass2(ChainSendParams P, ChainWideScratch W) {
+  __shared__ float buf[kWideT][kWideLc + 1];
+  __shared__ double V[kChainStates * kWideT];
+  __shared__ double PW[kWideLogT][kChainStates][kChainStates];
+  const int ch = blockIdx.y, b = blockIdx.x, t = threadIdx.x;
+  const long long base = (long long)b * kWideSpan;
+  chain_wide_stage(P, ch, base, buf);
+  if (P.lc.on || P.hc.on) {
+    for (int j = t; j < kWideLogT * kChainStates * kChainStates; j += kWideT) (&PW[0][0][0])[j] = W.pw[j];
+    const float* z = W.z + (((long long)ch * W.nb_cap + b) * kWideT + t) * kChainStates;
+#pragma unroll
+    for (int q = 0; q < kChainStates; ++q) V[q * kWideT + t] = z[q];
+    __syncthreads();
+    double G[kChainStates] = {0, 0, 0, 0, 0, 0, 0, 0};
+    if (t == 0) {                       // seed: V[0] = M G_b + Z_0, so that V[t] becomes the state after chunk t
+      const double* g = W.carry + ((long long)ch * W.nb_cap + b) * kChainStates;
+      double acc[kChainStates];
+#pragma unroll
+      for (int q = 0; q < kChainStates; ++q) { G[q] = g[q]; acc[q] = V[q * kWideT]; }
+      chain_affine_acc(PW[0], G, acc);
+#pragma unroll
+      for (int q = 0; q < kChainStates; ++q) V[q * kWideT] = acc[q];
+    }
+    __syncthreads();
+    chain_wide_scan<kWideT>(PW, V);
+    float s[kChainStates];
+#pragma unroll
+    for (int q = 0; q < kChainStates; ++q) s[q] = (float)(t == 0 ? G[q] : V[q * kWideT + t - 1]);
+    const long long i0 = base + (long long)t * kWideLc;
+    const int m = chain_wide_len(P.n, i0);
+    for (int k = 0; k < m; ++k) buf[t][k] = chain_cascade<float>(P, s, buf[t][k]);
+    if (m > 0 && i0 + m == P.n) {       // the state after the piece's last sample
+#pragma unroll
+      for (int q = 0; q < kChainStates; ++q) P.state[ch * kChainStateStride + q] = s[q];
+    }
+  }
+  __syncthreads();
+  for (int j = t; j < kWideSpan; j += kWideT) {
+    const long long i = base + j;
+    if (i < P.n) chain_wide_store(P, ch, i, buf[j / kWideLc][j % kWideLc]);
+  }
+}
 #else
 // CPU emulation (tests/emu): same chunking, same two passes
 inline void emu_chain_send(const ChainSendParams& P, int T) {
@@ -334,6 +583,120 @@ inline void emu_chain_send(const ChainSendParams& P, int T) {
     for (long long i = 0; i < P.n; ++i) chain_ring_write(P, ch, i);
     for (long long i = 0; i < P.n; ++i) chain_ring_read(P, ch, i);
   }
+}
+// the whole-GPU send form: the same chunking, reduction tree and scan order, one CTA / thread after another
+inline void emu_chain_wide_scan(const double (*Mj)[kChainStates][kChainStates], double* V, int N) {
+  double* nx = new double[(size_t)N * kChainStates];
+  for (int j = 0, d = 1; d < N; ++j, d *= 2) {
+    for (int t = d; t < N; ++t) chain_combine(Mj[j], V, N, t, d, false, nx + (size_t)t * kChainStates);
+    for (int t = d; t < N; ++t)
+      for (int q = 0; q < kChainStates; ++q) V[q * N + t] = nx[(size_t)t * kChainStates + q];
+  }
+  delete[] nx;
+}
+inline void emu_chain_wide(const ChainSendParams& P, const ChainWideScratch& W, bool powers) {
+  const bool filtered = P.lc.on || P.hc.on;
+  const long long nb = chain_wide_ctas(P.n);
+  constexpr int S2 = kChainStates * kChainStates;
+  if (filtered && powers) {
+    double M[kChainStates][kChainStates], nx[kChainStates][kChainStates];
+    for (int j = 0; j < kChainStates; ++j) {
+      double col[kChainStates];
+      chain_power_column(P, 1, j, col);
+      for (int k = 0; k < kChainStates; ++k) M[k][j] = col[k];
+    }
+    for (int s = 1; s < kWideLogLc + kWidePowers; ++s) {
+      for (int q = 0; q < kChainStates; ++q)
+        for (int r = 0; r < kChainStates; ++r) nx[q][r] = chain_square_entry(M, q, r);
+      for (int q = 0; q < kChainStates; ++q)
+        for (int r = 0; r < kChainStates; ++r) {
+          M[q][r] = nx[q][r];
+          if (s >= kWideLogLc) W.pw[(s - kWideLogLc) * S2 + q * kChainStates + r] = nx[q][r];
+        }
+    }
+  }
+  const double (*PW)[kChainStates][kChainStates] = reinterpret_cast<const double (*)[kChainStates][kChainStates]>(W.pw);
+  float (*buf)[kWideLc + 1] = new float[kWideT][kWideLc + 1];
+  double* V = new double[(size_t)kChainStates * kWideCarryT];
+  auto stage = [&](int ch, long long base) {
+    for (int j = 0; j < kWideSpan; ++j) {
+      const long long i = base + j;
+      buf[j / kWideLc][j % kWideLc] = i < P.n ? chain_wide_send(P, ch, i) : 0.0f;
+    }
+  };
+  auto len = [&](long long i0) { return i0 >= P.n ? 0 : (P.n - i0 < kWideLc ? (int)(P.n - i0) : kWideLc); };
+  if (filtered) {
+    for (int ch = 0; ch < 2; ++ch)                 // pass 1
+      for (long long b = 0; b < nb; ++b) {
+        const long long base = b * kWideSpan;
+        stage(ch, base);
+        for (int t = 0; t < kWideT; ++t) {
+          float s[kChainStates] = {0, 0, 0, 0, 0, 0, 0, 0};
+          const int m = len(base + (long long)t * kWideLc);
+          for (int k = 0; k < m; ++k) (void)chain_cascade<float>(P, s, buf[t][k]);
+          float* z = W.z + (((long long)ch * W.nb_cap + b) * kWideT + t) * kChainStates;
+          for (int q = 0; q < kChainStates; ++q) { z[q] = s[q]; V[q * kWideT + t] = s[q]; }
+        }
+        for (int j = 0, d = 1; d < kWideT; ++j, d *= 2)
+          for (int t = 0; t < kWideT; t += 2 * d) {
+            double nx[kChainStates];
+            chain_combine(PW[j], V, kWideT, t, d, true, nx);
+            for (int q = 0; q < kChainStates; ++q) V[q * kWideT + t] = nx[q];
+          }
+        for (int q = 0; q < kChainStates; ++q) W.agg[((long long)ch * W.nb_cap + b) * kChainStates + q] = V[q * kWideT];
+      }
+    for (int ch = 0; ch < 2; ++ch) {               // carry
+      double c[kChainStates];
+      chain_scan_start(P, ch, c);
+      const double* agg = W.agg + (long long)ch * W.nb_cap * kChainStates;
+      double* G = W.carry + (long long)ch * W.nb_cap * kChainStates;
+      for (long long g0 = 0; g0 < nb; g0 += kWideCarryT - 1) {
+        for (int t = 0; t < kWideCarryT; ++t) {
+          const long long a = g0 + t - 1;
+          for (int q = 0; q < kChainStates; ++q)
+            V[q * kWideCarryT + t] = t == 0 ? c[q] : (a < nb - 1 ? agg[a * kChainStates + q] : 0.0);
+        }
+        emu_chain_wide_scan(PW + kWideLogT, V, kWideCarryT);
+        for (int t = 0; t < kWideCarryT && g0 + t < nb; ++t)
+          for (int q = 0; q < kChainStates; ++q) G[(g0 + t) * kChainStates + q] = V[q * kWideCarryT + t];
+        for (int q = 0; q < kChainStates; ++q) c[q] = V[q * kWideCarryT + kWideCarryT - 1];
+      }
+    }
+  }
+  for (int ch = 0; ch < 2; ++ch)                   // pass 2
+    for (long long b = 0; b < nb; ++b) {
+      const long long base = b * kWideSpan;
+      stage(ch, base);
+      if (filtered) {
+        for (int t = 0; t < kWideT; ++t) {
+          const float* z = W.z + (((long long)ch * W.nb_cap + b) * kWideT + t) * kChainStates;
+          for (int q = 0; q < kChainStates; ++q) V[q * kWideT + t] = z[q];
+        }
+        double G[kChainStates], acc[kChainStates];
+        for (int q = 0; q < kChainStates; ++q) {
+          G[q] = W.carry[((long long)ch * W.nb_cap + b) * kChainStates + q];
+          acc[q] = V[q * kWideT];
+        }
+        chain_affine_acc(PW[0], G, acc);
+        for (int q = 0; q < kChainStates; ++q) V[q * kWideT] = acc[q];
+        emu_chain_wide_scan(PW, V, kWideT);
+        for (int t = 0; t < kWideT; ++t) {
+          float s[kChainStates];
+          for (int q = 0; q < kChainStates; ++q) s[q] = (float)(t == 0 ? G[q] : V[q * kWideT + t - 1]);
+          const long long i0 = base + (long long)t * kWideLc;
+          const int m = len(i0);
+          for (int k = 0; k < m; ++k) buf[t][k] = chain_cascade<float>(P, s, buf[t][k]);
+          if (m > 0 && i0 + m == P.n)
+            for (int q = 0; q < kChainStates; ++q) P.state[ch * kChainStateStride + q] = s[q];
+        }
+      }
+      for (int j = 0; j < kWideSpan; ++j) {
+        const long long i = base + j;
+        if (i < P.n) chain_wide_store(P, ch, i, buf[j / kWideLc][j % kWideLc]);
+      }
+    }
+  delete[] buf;
+  delete[] V;
 }
 inline void emu_chain_wet(const ChainWetParams& P) {
   for (long long i = 0; i < P.n; ++i) chain_wet_sample(P, i);
