@@ -242,6 +242,37 @@ int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* 
 int b200conv_chain_process_device(b200conv_t* h, const float* dry_dev, size_t dry_stride, const float* ysend_dev,
                                   const float* yrev_dev, float* out_dev, size_t out_stride, size_t len, int sync);
 
+/* b200conv_chain_process_device with parameter changes at sample offsets inside the call, for renders with automation
+ * of the low / high cut, predelay, width, dry / wet gain or true stereo (the envelopes already vary per sample).
+ * events[i].cfg takes effect at sample events[i].offset of the call.  The output equals, within float rounding, the
+ * call cut at every event offset into consecutive b200conv_chain_process_device calls with
+ * b200conv_chain_update(h, &events[i].cfg) made just before the call that starts at events[i].offset; everything
+ * b200conv_chain_update documents holds per event, at that sample (filter states continue, the 6 dB and 12 / 24 dB
+ * state variables are kept across slope switches, a filter switched off keeps its state, the delay line is read at
+ * the new predelay, and a predelay beyond D sets D = 2 * predelay with the delay history reading zero from that
+ * sample on).  Afterwards the handle's configuration is the last event's.
+ * events: host memory, read during the call; offsets strictly increasing and below len.  n_events == 0 is
+ * b200conv_chain_process_device exactly (events may then be NULL).  Every event is checked before anything is
+ * enqueued; on any error nothing changes.  Asynchronous like b200conv_chain_process_device, except that a predelay
+ * whose D outgrows the device ring reallocates the ring once, before the first launch (synchronising the handle's
+ * stream, as b200conv_chain_update does).  The first call that needs them allocates the segmented send form's
+ * scratch (sized for the handle's batch) and a table of one row per event; a call with more events than any before
+ * grows the table; both happen before the call's first launch.  A call waits for the previous events call's table
+ * copy (the start of that call's work on the stream) before it rewrites the table's staging.
+ * The convolvers run the pieces of b200conv_chain_process_device unchanged; the send filters of a long piece over
+ * several events run a segmented form of the whole-GPU scan.
+ * B200CONV_ESTATE: no chain, a fixed-latency handle, or an IR hot swap pending (b200conv_chain_swap_state 1 or 2).
+ * B200CONV_EINVAL: dry_dev or out_dev NULL, events NULL with n_events > 0, or a bad event (b200conv_chain_update's
+ * rules, an srate other than the configured one, offsets out of order or not below len). */
+typedef struct b200conv_chain_event {
+  size_t offset;                /* sample of the call at which cfg takes effect, 0 <= offset < len */
+  b200conv_chain_config cfg;    /* the struct b200conv_chain_update takes */
+} b200conv_chain_event;
+int b200conv_chain_process_device_events(b200conv_t* h, const float* dry_dev, size_t dry_stride,
+                                         const float* ysend_dev, const float* yrev_dev, float* out_dev,
+                                         size_t out_stride, size_t len, const b200conv_chain_event* events,
+                                         size_t n_events, int sync);
+
 /* IR hot-swap inside the device chain (src/PluginProcessor.cpp:1655-1668, 1694-1756, 1799-1830).
  * `live` has the chain configured; `incoming` holds the new IR (e.g. b200conv_init_twostage_recalc).
  * The next b200conv_chain_process(live, ...) does the warm-up (0.25 s of send history, replayed on the device in

@@ -31,6 +31,10 @@ class ChainConfig(C.Structure):
                 ("wetgain", C.c_float), ("true_stereo", C.c_int)]
 
 
+class ChainEvent(C.Structure):
+    _fields_ = [("offset", C.c_size_t), ("cfg", ChainConfig)]
+
+
 class IrShapeParams(C.Structure):
     _fields_ = [("autogain", C.c_int), ("reverse", C.c_int), ("trim_left", C.c_float), ("trim_right", C.c_float),
                 ("gain", C.c_float), ("decay_lut", C.c_void_p), ("srate", C.c_double), ("clip", C.c_int),
@@ -108,6 +112,9 @@ SYMBOLS = [
     ("b200conv_chain_process", C.c_int, [C.c_void_p, _PP, C.c_void_p, C.c_void_p, _PP, C.c_size_t]),
     ("b200conv_chain_process_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.c_size_t, C.c_size_t, C.c_int]),
+    ("b200conv_chain_process_device_events", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                                        C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t,
+                                                        C.c_int]),
     ("b200conv_chain_update", C.c_int, [C.c_void_p, C.c_void_p]),
     ("b200conv_chain_swap", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     ("b200conv_chain_swap_state", C.c_int, [C.c_void_p]),

@@ -29,6 +29,22 @@ def _ptr_array(arrs: Sequence[np.ndarray]):
     return arr
 
 
+def chain_event_array(events):
+    """[(offset, dict of chain_update's keywords), ...] as the b200conv_chain_event array Engine.chain_process_device_events
+    passes to the library"""
+    arr = (_lib.ChainEvent * len(events))()
+    for k, (off, kw) in enumerate(events):
+        kw = dict(kw)
+        ts = int(kw.pop("true_stereo", True))
+        arr[k].offset = int(off)
+        arr[k].cfg = _lib.ChainConfig(kw.pop("srate"), kw.pop("lowcut_hz", 20.0), kw.pop("lowcut_slope", 0),
+                                      kw.pop("highcut_hz", 20000.0), kw.pop("highcut_slope", 0), kw.pop("predelay", 0),
+                                      kw.pop("width", 1.0), kw.pop("drygain", 1.0), kw.pop("wetgain", 1.0), ts)
+        if kw:
+            raise TypeError(f"unknown chain parameters {sorted(kw)}")
+    return arr
+
+
 class Engine:
     """C mono convolvers in one handle (b200conv_t)."""
 
@@ -220,6 +236,17 @@ class Engine:
         mean 1.  Asynchronous on the handle's stream unless sync."""
         self._check(self._l.b200conv_chain_process_device(self._h, dry_ptr, dry_stride, ysend_ptr or None, yrev_ptr or None,
                                                           out_ptr, out_stride, n, int(sync)), "chain_process_device")
+
+    def chain_process_device_events(self, dry_ptr: int, dry_stride: int, out_ptr: int, out_stride: int, n: int, events,
+                                    ysend_ptr: int = 0, yrev_ptr: int = 0, sync: bool = False):
+        """chain_process_device with parameter changes inside the call (b200conv_chain_process_device_events):
+        events = [(offset, dict of chain_update's keywords), ...], offsets strictly increasing and below n, or an
+        array from chain_event_array (built once, reused by calls with the same automation); each configuration takes
+        effect at its sample, as chain_update before a call cut there would."""
+        arr = events if isinstance(events, C.Array) else chain_event_array(events)
+        self._check(self._l.b200conv_chain_process_device_events(
+            self._h, dry_ptr, dry_stride, ysend_ptr or None, yrev_ptr or None, out_ptr, out_stride, n,
+            C.cast(arr, C.c_void_p) if len(arr) else None, len(arr), int(sync)), "chain_process_device_events")
 
     def chain_swap(self, incoming: "Engine", host_block: int) -> None:
         """IR hot swap inside the chain (b200conv_chain_swap): the next chain_process call replays the send history

@@ -176,6 +176,15 @@ struct b200conv {
                                      // quad handle being crossfaded in)
   float* c_state = nullptr;          // [4][kChainStateStride] filter states: rows 0-1 the send, rows 2-3 the warm-up replay of a swap
   void* c_wide = nullptr;            // scratch of the whole-GPU send form (pc::ChainWideScratch), sized for Lmax
+  // parameter events inside device calls (b200conv_chain_process_device_events), allocated by the first call that needs
+  // them and grown before a call's first launch: the segmented send form's scratch (pc::ChainSegScratch, sized for
+  // Lmax), the call's segment table on the device and its pinned staging, and the event that ends the table's copy
+  void* c_seg = nullptr;
+  pc::ChainSeg* c_segtab = nullptr;
+  pc::ChainSeg* c_segpin = nullptr;
+  size_t c_segcap = 0;
+  cudaEvent_t c_segev = nullptr;
+  bool c_segev_live = false;
   bool c_six[2] = {false, false};    // slot 0 of the low / high cut's state holds the 6 dB `state` (else ic1)
   float* c_hpin = nullptr;           // pinned [dry L, dry R, ysend, yrev, out L, out R][hpin_cap]: zero-copy I/O of real-time chain calls
   float* c_hpin_dev = nullptr;
@@ -379,6 +388,10 @@ void free_all(b200conv* h) {
   h->tc_err = h->tc_err_dev = nullptr; h->tc_alloc_failed = false;
   cudaFree(h->c_io); cudaFree(h->c_conv_in); cudaFree(h->c_filt); cudaFree(h->c_state); cudaFree(h->c_ring);
   cudaFree(h->c_wide); h->c_wide = nullptr;
+  cudaFree(h->c_seg); cudaFree(h->c_segtab);
+  if (h->c_segpin) cudaFreeHost(h->c_segpin);
+  if (h->c_segev) cudaEventDestroy(h->c_segev);
+  h->c_seg = nullptr; h->c_segtab = h->c_segpin = nullptr; h->c_segcap = 0; h->c_segev = nullptr; h->c_segev_live = false;
   if (h->c_hpin) cudaFreeHost(h->c_hpin);
   h->c_hpin = h->c_hpin_dev = nullptr;
   h->c_io = h->c_conv_in = h->c_filt = h->c_state = h->c_ring = nullptr;
@@ -2993,6 +3006,48 @@ int launch_chain_wide(b200conv* h, const pc::ChainSendParams& sp, bool powers, c
   return 0;
 }
 
+// the segmented form's scratch inside one allocation of chain_seg_bytes(Lmax): P_j and M_b per CTA, T_c per chunk,
+// aggregates, carries, Z_c
+size_t chain_seg_bytes(size_t Lmax) {
+  const size_t nb = (size_t)pc::chain_wide_ctas((long long)Lmax), S = pc::kSegStates, S8 = pc::kChainStates;
+  return (nb * pc::kWideLogT * S8 * S8 + nb * S * S + nb * pc::kWideT * S * S + 4 * nb * S) * sizeof(double) +
+         2 * nb * pc::kWideT * S * sizeof(float);
+}
+pc::ChainSegScratch chain_seg_scratch(const b200conv* h) {
+  pc::ChainSegScratch w{};
+  const long long nb = pc::chain_wide_ctas((long long)h->Lmax), S = pc::kSegStates, S8 = pc::kChainStates;
+  w.nb_cap = nb;
+  w.pw = static_cast<double*>(h->c_seg);
+  w.mb = w.pw + nb * pc::kWideLogT * S8 * S8;
+  w.tc = w.mb + nb * S * S;
+  w.agg = w.tc + nb * pc::kWideT * S * S;
+  w.carry = w.agg + 2 * nb * S;
+  w.z = reinterpret_cast<float*>(w.carry + 2 * nb * S);
+  return w;
+}
+
+// the segmented whole-GPU send form of one piece that spans several rows of the segment table, and the predelayed
+// convolver input read from the ring after it
+int launch_chain_seg(b200conv* h, const pc::ChainSendParams& sp, const pc::ChainSegs& S, cudaStream_t st) {
+  const pc::ChainSegScratch w = chain_seg_scratch(h);
+#if defined(PC_EMULATE)
+  (void)st;
+  pc::emu_chain_seg(sp, S, w);
+  pc::emu_chain_seg_read(sp, S);
+#else
+  const long long nb = pc::chain_wide_ctas(sp.n);
+  const dim3 grid((unsigned)nb, 2);
+  pc::k_chain_seg_maps<<<(unsigned)nb, pc::kWideT, 0, st>>>(S, sp.n, w);
+  pc::k_chain_seg_pass1<<<grid, pc::kWideT, 0, st>>>(sp, S, w);
+  pc::k_chain_seg_carry<<<2, 32, 0, st>>>(sp, w, nb);
+  pc::k_chain_seg_pass2<<<grid, pc::kWideT, 0, st>>>(sp, S, w);
+  pc::k_chain_seg_read<<<dim3((unsigned)((sp.n + 255) / 256), 2), 256, 0, st>>>(sp, S);
+  CU_CHECK(h, cudaGetLastError());
+#endif
+  h->launches += 5;
+  return 0;
+}
+
 // Filter::init (src/dsp/Filter.cpp:3-21) with the q the processor passes (src/PluginProcessor.cpp:845-848)
 pc::ChainFilter chain_filter(bool on, int slope, int mode, float srate, float freq) {
   pc::ChainFilter f{};
@@ -3036,11 +3091,9 @@ size_t chain_ring_len(const b200conv* h, long long D) {
   return next_pow2(std::max((size_t)D, chain_warmer_len(h->chain_cfg.srate)) + h->Lmax + 1);
 }
 
-// delayBuffer.setSize(2, predelay * 2) + clear() + delaypos = 0 (src/PluginProcessor.cpp:1184-1188): the delay history
-// reads zero from here on (delay floor), but the samples stay in the ring, which is also the warmer (a separate buffer
-// in the reference that the growth does not touch).  A ring too short for the new D is reallocated, the samples it
-// holds carried over to their new positions.  The only chain parameter change that allocates and synchronises.
-int chain_grow_delay(b200conv* h, long long D) {
+// A ring too short for a delay line of D samples is reallocated, the samples it holds carried over to their new
+// positions.  The only chain parameter change that allocates and synchronises.
+int chain_grow_ring(b200conv* h, long long D) {
   const size_t ring = chain_ring_len(h, D);
   if (ring > h->c_ring_size) {
     if (int rc = set_device(h)) return rc;
@@ -3064,6 +3117,13 @@ int chain_grow_delay(b200conv* h, long long D) {
     cudaFree(h->c_ring);
     h->c_ring = nr; h->c_ring_size = ring;
   }
+  return 0;
+}
+// delayBuffer.setSize(2, predelay * 2) + clear() + delaypos = 0 (src/PluginProcessor.cpp:1184-1188): the delay history
+// reads zero from here on (delay floor), but the samples stay in the ring, which is also the warmer (a separate buffer
+// in the reference that the growth does not touch)
+int chain_grow_delay(b200conv* h, long long D) {
+  if (int rc = chain_grow_ring(h, D)) return rc;
   h->c_delay_len = D;
   h->c_delay_floor = h->c_ring_pos;
   return 0;
@@ -3271,6 +3331,69 @@ int chain_piece(b200conv* h, const float* d_dry, const float* d_send, const floa
   h->launches++;
   return 0;
 }
+
+// One piece of a device call with parameter events: the call's samples [off, off + n), which rows [lo, hi) of the
+// segment table overlap (rows: the host copy, d_rows: the device copy).  Long pieces inside one row run the whole-GPU
+// form with that row (*powered: the row whose P_j the scratch holds), long pieces over several rows the segmented form,
+// short pieces k_chain_send once per row.  No swap is pending (the entry refuses events then).
+int chain_piece_events(b200conv* h, const pc::ChainSeg* rows, const pc::ChainSeg* d_rows, int lo, int hi, size_t off,
+                       const float* d_dry, const float* d_send, const float* d_rev, float* d_out, size_t dry_stride,
+                       size_t out_stride, size_t n, int* powered) {
+  const size_t L = h->Lmax;
+  pc::ChainSendParams sp{};
+  sp.dry = d_dry; sp.dry_stride = (long long)dry_stride; sp.ysend = d_send;
+  sp.conv_in = h->c_conv_in; sp.conv_stride = (long long)L;
+  sp.filt = h->c_filt; sp.filt_stride = (long long)L;
+  sp.state = h->c_state;
+  sp.ring = h->c_ring; sp.ring_stride = (long long)h->c_ring_size; sp.ring_mask = (long long)h->c_ring_size - 1;
+  sp.ring_pos = h->c_ring_pos;
+  sp.n = (long long)n;
+  const pc::ChainSegs S{d_rows + lo, hi - lo, (long long)off};
+  if (n >= kChainWideMin && hi - lo > 1) {
+    sp.filt = nullptr;
+    if (int rc = launch_chain_seg(h, sp, S, h->s_main)) return rc;
+  } else {
+    for (int k = lo; k < hi; ++k) {             // the part of the piece in row k, as the cut call would run it
+      const pc::ChainSeg& g = rows[k];
+      const size_t a = std::max((size_t)g.start, off) - off;
+      const size_t b = (k + 1 < hi ? (size_t)rows[k + 1].start : off + n) - off;
+      pc::ChainSendParams p = sp;
+      p.dry = d_dry + a; p.ysend = d_send ? d_send + a : nullptr;
+      p.conv_in = sp.conv_in + a; p.filt = sp.filt + a;
+      p.ring_pos = sp.ring_pos + (long long)a; p.n = (long long)(b - a);
+      p.lc = g.lc; p.hc = g.hc;
+      p.predelay = g.predelay; p.delay_floor = g.delay_floor;
+      const bool starts = (size_t)g.start == off + a;
+      p.swap_lc = starts ? g.swap_lc : 0; p.swap_hc = starts ? g.swap_hc : 0;
+      if (n >= kChainWideMin) {
+        p.filt = nullptr;
+        if (int rc = launch_chain_wide(h, p, *powered != k, h->s_main)) return rc;
+        if (p.lc.on || p.hc.on) *powered = k;
+      } else if (int rc = launch_chain_send(h, p, h->s_main)) {
+        return rc;
+      }
+    }
+  }
+  h->c_ring_pos += (long long)n;
+  if (int rc = chain_convolve(h, h->c_conv_in, L, n)) return rc;
+  pc::ChainWetParams wp{};
+  wp.dry = d_dry; wp.dry_stride = (long long)dry_stride;
+  wp.conv = h->dch[0]; wp.conv_stride = (long long)L;
+  wp.yrev = d_rev;
+  wp.out = d_out; wp.out_stride = (long long)out_stride; wp.n = (long long)n;
+  const pc::ChainSeg& g = rows[lo];
+  wp.quad_ts = g.quad_ts; wp.width = g.width; wp.drygain = g.drygain; wp.wetgain = g.wetgain;
+#if defined(PC_EMULATE)
+  if (hi - lo > 1) pc::emu_chain_wet_seg(wp, S);
+  else pc::emu_chain_wet(wp);
+#else
+  if (hi - lo > 1) pc::k_chain_wet_seg<<<(unsigned)((n + 255) / 256), 256, 0, h->s_main>>>(wp, S);
+  else pc::k_chain_wet<<<(unsigned)((n + 255) / 256), 256, 0, h->s_main>>>(wp);
+  CU_CHECK(h, cudaGetLastError());
+#endif
+  h->launches++;
+  return 0;
+}
 }  // namespace
 
 // A chain call in fixed-latency mode: one step per head block, each the zero-latency chain piece of B0 samples with the
@@ -3382,6 +3505,107 @@ int b200conv_chain_process_device(b200conv_t* h, const float* dry_dev, size_t dr
     CU_CHECK(h, cudaEventRecord(h->ev_h2d[0], h->s_main));
     CU_CHECK(g, cudaStreamWaitEvent(g->s_main, h->ev_h2d[0], 0));
   }
+  if (sync) CU_CHECK(h, cudaStreamSynchronize(h->s_main));
+  return B200CONV_OK;
+}
+
+// The device chain with parameter events: the call keeps b200conv_chain_process_device's pieces and convolver calls and
+// carries the parameters as a table of rows, one per stretch of samples with one configuration.  Everything is
+// checked first; the delay line grows once to the largest D the events reach; the table goes to the device in one
+// copy; the handle ends with the last event's configuration, as after the equivalent b200conv_chain_update calls.
+int b200conv_chain_process_device_events(b200conv_t* h, const float* dry_dev, size_t dry_stride, const float* ysend_dev,
+                                         const float* yrev_dev, float* out_dev, size_t out_stride, size_t len,
+                                         const b200conv_chain_event* events, size_t n_events, int sync) {
+  REQUIRE_CUDA(h);
+  if (n_events == 0)
+    return b200conv_chain_process_device(h, dry_dev, dry_stride, ysend_dev, yrev_dev, out_dev, out_stride, len, sync);
+  if (!h->chain_on) return fail(h, B200CONV_ESTATE, "b200conv_chain_configure first");
+  if (h->lat_D) return fail(h, B200CONV_ESTATE, "device-pointer calls are not available in fixed-latency mode");
+  if (h->swap_peer) return fail(h, B200CONV_ESTATE, "parameter events are not available while an IR hot swap is pending");
+  if (h->stages.empty()) return fail(h, B200CONV_ESTATE, "no impulse response loaded");
+  if (!dry_dev || !out_dev || !events) return fail(h, B200CONV_EINVAL, "null buffer");
+  for (size_t i = 0; i < n_events; ++i) {
+    const b200conv_chain_event& ev = events[i];
+    if (!chain_config_ok(ev.cfg) || ev.cfg.srate != h->chain_cfg.srate)
+      return fail(h, B200CONV_EINVAL, "bad chain configuration in an event");
+    if (ev.offset >= len || (i > 0 && ev.offset <= events[i - 1].offset))
+      return fail(h, B200CONV_EINVAL, "event offsets must increase strictly and stay below len");
+  }
+  if (int rc = set_device(h)) return rc;
+  // the rows: the current configuration up to the first event, then one per event, with the slope exchanges and the
+  // delay floors the equivalent b200conv_chain_update calls would leave
+  std::vector<pc::ChainSeg> rows;
+  rows.reserve(n_events + 1);
+  bool six[2] = {h->c_six[0], h->c_six[1]};
+  long long D = h->c_delay_len, floor = h->c_delay_floor;
+  auto add = [&](const b200conv_chain_config& cfg, size_t start) {
+    pc::ChainSeg g{};
+    g.start = (long long)start;
+    const float sr = (float)cfg.srate;
+    g.lc = chain_filter(cfg.lowcut_hz > 20.0f, cfg.lowcut_slope, 2, sr, cfg.lowcut_hz);
+    g.hc = chain_filter(cfg.highcut_hz < 20000.0f, cfg.highcut_slope, 0, sr, cfg.highcut_hz);
+    if (g.lc.on || g.hc.on) {
+      g.swap_lc = six[0] != (g.lc.slope == 0); g.swap_hc = six[1] != (g.hc.slope == 0);
+      six[0] = g.lc.slope == 0; six[1] = g.hc.slope == 0;
+    }
+    const long long nD = chain_delay_len(D, cfg.predelay);
+    if (nD != D) { D = nD; floor = h->c_ring_pos + (long long)start; }
+    g.delay_floor = floor;
+    g.predelay = cfg.predelay;
+    g.quad_ts = (h->C == 4 && cfg.true_stereo) ? 1 : 0;
+    g.width = cfg.width; g.drygain = cfg.drygain; g.wetgain = cfg.wetgain;
+    rows.push_back(g);
+  };
+  if (events[0].offset > 0) add(h->chain_cfg, 0);
+  for (size_t i = 0; i < n_events; ++i) add(events[i].cfg, events[i].offset);
+  // allocations, before the first launch: the delay line (synchronising, as b200conv_chain_update does), the segmented
+  // form's scratch, the table and its staging (the first call that needs them, or a longer table)
+  if (D != h->c_delay_len)
+    if (int rc = chain_grow_ring(h, D)) return rc;
+  const size_t L = h->Lmax, B0 = h->stages[0].B, chunk = L - B0;
+  const int nrows = (int)rows.size();
+  // the pieces: samples [done, done + n) of the call overlap rows [lo, hi)
+  struct Piece { size_t done, n; int lo, hi; };
+  std::vector<Piece> pieces;
+  bool segmented = false;
+  for (size_t done = 0, lo = 0; done < len;) {
+    const size_t n = std::min(len - done, chunk);
+    while ((int)lo + 1 < nrows && (size_t)rows[lo + 1].start <= done) ++lo;
+    size_t hi = lo + 1;
+    while ((int)hi < nrows && (size_t)rows[hi].start < done + n) ++hi;
+    pieces.push_back({done, n, (int)lo, (int)hi});
+    segmented |= n >= kChainWideMin && hi - lo > 1;
+    done += n;
+  }
+  if (segmented && !h->c_seg) CU_CHECK(h, cudaMalloc(&h->c_seg, chain_seg_bytes(L)));
+  if (rows.size() > h->c_segcap) {
+    const size_t cap = std::max(rows.size(), 2 * h->c_segcap);
+    cudaFree(h->c_segtab); h->c_segtab = nullptr;
+    if (h->c_segpin) cudaFreeHost(h->c_segpin);
+    h->c_segpin = nullptr; h->c_segcap = 0; h->c_segev_live = false;
+    CU_CHECK(h, cudaMalloc(&h->c_segtab, cap * sizeof(pc::ChainSeg)));
+    CU_CHECK(h, cudaMallocHost((void**)&h->c_segpin, cap * sizeof(pc::ChainSeg)));
+    h->c_segcap = cap;
+  }
+  if (!h->c_segev) CU_CHECK(h, cudaEventCreateWithFlags(&h->c_segev, cudaEventDisableTiming));
+#if !defined(PC_EMULATE)
+  // the staging is rewritten only after the previous events call's copy out of it (the head of that call's work)
+  if (h->c_segev_live) CU_CHECK(h, cudaEventSynchronize(h->c_segev));
+#endif
+  std::memcpy(h->c_segpin, rows.data(), rows.size() * sizeof(pc::ChainSeg));
+  CU_CHECK(h, cudaMemcpyAsync(h->c_segtab, h->c_segpin, rows.size() * sizeof(pc::ChainSeg), cudaMemcpyHostToDevice,
+                              h->s_main));
+  CU_CHECK(h, cudaEventRecord(h->c_segev, h->s_main));
+  h->c_segev_live = true;
+  int powered = -1;
+  for (const Piece& p : pieces)
+    if (int rc = chain_piece_events(h, rows.data(), h->c_segtab, p.lo, p.hi, p.done, dry_dev + p.done,
+                                    ysend_dev ? ysend_dev + p.done : nullptr, yrev_dev ? yrev_dev + p.done : nullptr,
+                                    out_dev + p.done, dry_stride, out_stride, p.n, &powered)) return rc;
+  h->chain_cfg = events[n_events - 1].cfg;
+  chain_set_filters(h, h->chain_cfg);
+  h->c_delay_len = D; h->c_delay_floor = floor;
+  h->c_six[0] = six[0]; h->c_six[1] = six[1];
   if (sync) CU_CHECK(h, cudaStreamSynchronize(h->s_main));
   return B200CONV_OK;
 }

@@ -307,6 +307,135 @@ PC_HD void chain_wide_store(const ChainSendParams& P, int ch, long long i, float
   if (P.filt) P.filt[(long long)ch * P.filt_stride + i] = y;
 }
 
+// ---- parameter events inside one device call (b200conv_chain_process_device_events) --------------------------------
+// The call carries a table of segments, one row per stretch of samples with one parameter set; a piece of the call
+// overlaps a contiguous run of rows.  A piece inside one row runs the kernels above with that row's parameters.  A long
+// piece that spans several rows runs the segmented whole-GPU form, in five launches:
+//   maps   k_chain_seg_maps: per CTA, either (uniform CTA: one row, no slope exchange at its first sample) the powers
+//          P_j = A^(kWideLc * 2^j) of that row's A, squared exactly as k_chain_wide_powers squares them, and
+//          M_b = P_kWideLogT; or (mixed CTA) every chunk's transfer matrix T_c from kSegStates zero-input runs in double
+//          over its samples, switching coefficients and exchanging slot 0 and the stash where a row starts, and
+//          M_b = T_last ... T_0 composed in order
+//   pass 1 k_chain_seg_pass1: every chunk from a zero state (FP32, switching as above) gives Z_c; a uniform CTA folds
+//          them by k_chain_wide_pass1's tree with its P_j, a mixed one by S <- T_c S + Z_c in double, in order
+//   carry  k_chain_seg_carry: G_{b+1} = M_b G_b + agg_b in double from the carried state, CTA after CTA
+//   pass 2 k_chain_seg_pass2: a uniform CTA seeds and scans as k_chain_wide_pass2 does; a mixed one runs
+//          S <- T_c S + Z_c from G_b; both re-run the chunks from the rounded seeds and write the ring
+//   read   k_chain_seg_read: the predelayed convolver input, each sample at its row's predelay and delay floor
+// The state is kSegStates wide: the 8 scan slots and the two stash slots, which only slope exchanges move (a
+// permutation, exact in double), so the stash a row leaves is the FP32 value the serial filter would leave.  The
+// double scan has the precision argument of the event-free form: every T_c and M_b is the exact-coefficient transfer
+// of its samples, rounded once per entry, and each chunk's seed is rounded to float once; nothing accumulates across
+// rows beyond the scan's own rounding.  The ring is read only after pass 2 has written the whole piece, in its own
+// launch: with a predelay that changes inside the piece, the sample a convolver input needs may belong to another CTA.
+// The slots it reads lie at most predelay + n - 1 < ring size behind every slot the piece writes, as in the event-free
+// form.
+constexpr int kSegStates = kChainStates + 2;
+
+struct ChainSeg {                  // one row: parameters from sample `start` of the call on
+  long long start;
+  long long delay_floor;           // absolute ring position below which the delay reads zero
+  ChainFilter lc, hc;
+  int swap_lc, swap_hc;            // the slope crossed 6 dB <-> 12 / 24 dB at `start`: slot 0 and the stash trade places
+  int predelay;
+  int quad_ts;
+  float width, drygain, wetgain;
+};
+
+struct ChainSegs {                 // the rows one piece overlaps
+  const ChainSeg* seg;             // the row in force at the piece's first sample
+  int nseg;
+  long long off;                   // the piece's first sample in the call
+};
+
+// scratch of the segmented form, sized for Lmax (grown by the first events call that needs it, before its first launch)
+struct ChainSegScratch {
+  double* pw;                      // [nb_cap][kWideLogT][8][8] P_j of uniform CTAs
+  double* mb;                      // [nb_cap][kSegStates][kSegStates] M_b
+  double* tc;                      // [nb_cap * kWideT][kSegStates][kSegStates] T_c of mixed CTAs
+  double* agg;                     // [2][nb_cap][kSegStates]
+  double* carry;                   // [2][nb_cap][kSegStates] G_b
+  float* z;                        // [2][nb_cap * kWideT][kSegStates] zero-state end points
+  long long nb_cap;
+};
+
+// samples of the chunk starting at sample i0 of an n-sample piece (0 .. kWideLc)
+PC_HD int chain_seg_len(long long n, long long i0) {
+  return i0 >= n ? 0 : (n - i0 < kWideLc ? (int)(n - i0) : kWideLc);
+}
+
+// the row in force at sample i of the piece
+PC_HD int chain_seg_at(const ChainSegs& S, long long i) {
+  const long long a = S.off + i;
+  int lo = 0, hi = S.nseg - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) / 2;
+    if (S.seg[mid].start <= a) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// the CTA [base, end) lies inside one row and starts with no slope exchange: that row, else -1
+PC_HD int chain_seg_uniform(const ChainSegs& S, long long base, long long end) {
+  const int k = chain_seg_at(S, base);
+  if (k + 1 < S.nseg && S.seg[k + 1].start < S.off + end) return -1;
+  if (S.seg[k].start == S.off + base && (S.seg[k].swap_lc || S.seg[k].swap_hc)) return -1;
+  return k;
+}
+
+// chain_cascade with a row's filters (the same arithmetic)
+template <class F>
+PC_HD F chain_seg_cascade(const ChainSeg& g, F* s, F x) {
+  if (g.lc.on) x = chain_filter_eval<F>(g.lc, s, x);
+  if (g.hc.on) x = chain_filter_eval<F>(g.hc, s + 4, x);
+  return x;
+}
+
+// m samples from sample i0 of the piece on the kSegStates-wide state s; x: input (nullptr: zeros), y: output or nullptr
+// (may be x).  Where a row starts, its slope exchange happens before its first sample.
+template <class F>
+PC_HD void chain_seg_run(const ChainSegs& S, long long i0, int m, F* s, const float* x, float* y) {
+  int k = chain_seg_at(S, i0);
+  for (int j = 0; j < m; ++j) {
+    const long long a = S.off + i0 + j;
+    if (k + 1 < S.nseg && S.seg[k + 1].start <= a) ++k;
+    const ChainSeg& g = S.seg[k];
+    if (g.start == a) {
+      if (g.swap_lc) { const F v = s[0]; s[0] = s[kChainStates]; s[kChainStates] = v; }
+      if (g.swap_hc) { const F v = s[4]; s[4] = s[kChainStates + 1]; s[kChainStates + 1] = v; }
+    }
+    const F v = chain_seg_cascade<F>(g, s, x ? (F)x[j] : (F)0);
+    if (y) y[j] = (float)v;
+  }
+}
+
+// column j of chunk c's transfer matrix T_c (a zero-input run from the unit state e_j)
+PC_HD void chain_seg_column(const ChainSegs& S, long long i0, int m, int j, double* col) {
+  for (int q = 0; q < kSegStates; ++q) col[q] = (q == j) ? 1.0 : 0.0;
+  chain_seg_run<double>(S, i0, m, col, nullptr, nullptr);
+}
+
+// the convolver input of sample i: the ring at the row's predelay, zero below the row's delay floor
+PC_HD void chain_seg_ring_read(const ChainSendParams& P, const ChainSeg& g, int ch, long long i) {
+  const long long p = P.ring_pos + i - g.predelay;
+  P.conv_in[(long long)ch * P.conv_stride + i] =
+      p < g.delay_floor ? 0.0f : P.ring[(long long)ch * P.ring_stride + (p & P.ring_mask)];
+}
+
+// chain_wet_mix with a row's width and gains
+PC_HD void chain_wet_seg_sample(const ChainWetParams& P, const ChainSeg& g, long long i) {
+  float wl = P.conv[i], wr = P.conv[P.conv_stride + i];
+  if (g.quad_ts) { wl += P.conv[3 * P.conv_stride + i]; wr += P.conv[2 * P.conv_stride + i]; }
+  const float e = P.yrev ? P.yrev[i] : 1.0f;
+  const float lin = wl * e, rin = wr * e;
+  const float mid = (lin + rin) * 0.5f, side = (lin - rin) * 0.5f;
+  const float norm = 1.0f / (1.0f + g.width);
+  const float lout = (mid + side * g.width) * norm;
+  const float rout = (mid - side * g.width) * norm;
+  P.out[i] = P.dry[i] * g.drygain + lout * g.wetgain;
+  P.out[P.out_stride + i] = P.dry[P.dry_stride + i] * g.drygain + rout * g.wetgain;
+}
+
 #if defined(__CUDACC__)
 // grid (2 channels), block T threads (T = 64 for real-time calls, 1024 for batches); static smem
 static __global__ void __launch_bounds__(1024) k_chain_send(ChainSendParams P) {
@@ -542,6 +671,247 @@ static __global__ void __launch_bounds__(kWideT) k_chain_wide_pass2(ChainSendPar
     if (i < P.n) chain_wide_store(P, ch, i, buf[j / kWideLc][j % kWideLc]);
   }
 }
+
+// segmented whole-GPU send form (see above).  S <- T_c S + V[., c] for the CTA's chunks in order, thread q < kSegStates
+// one row; `seeds`: V[q][c] becomes S[q] entering chunk c.  Sv: S in shared memory
+static __device__ __forceinline__ void chain_seg_serial(const double* tc, double* V, double* Sv, bool seeds) {
+  const int q = threadIdx.x;
+#pragma unroll 1
+  for (int c = 0; c < kWideT; ++c) {
+    double a = 0.0;
+    if (q < kSegStates) {
+      a = V[q * kWideT + c];
+      if (seeds) V[q * kWideT + c] = Sv[q];
+      const double* row = tc + ((long long)c * kSegStates + q) * kSegStates;
+#pragma unroll
+      for (int r = 0; r < kSegStates; ++r) a = fma(row[r], Sv[r], a);
+    }
+    __syncthreads();
+    if (q < kSegStates) Sv[q] = a;
+    __syncthreads();
+  }
+}
+
+// maps: per CTA the powers of its row (uniform) or its chunks' T_c and their product (mixed).  grid (CTAs)
+static __global__ void __launch_bounds__(kWideT) k_chain_seg_maps(ChainSegs S, long long n, ChainSegScratch W) {
+  __shared__ double M[kSegStates][kSegStates];
+  const int b = blockIdx.x, t = threadIdx.x;
+  const long long base = (long long)b * kWideSpan, end = base + kWideSpan < n ? base + kWideSpan : n;
+  const int k = chain_seg_uniform(S, base, end);
+  double* mb = W.mb + (long long)b * kSegStates * kSegStates;
+  if (k >= 0) {                         // k_chain_wide_powers' squarings, P_0 .. P_kWideLogT
+    const int q = t / kChainStates, r = t % kChainStates;
+    if (t < kChainStates) {
+      double col[kChainStates];
+      for (int p = 0; p < kChainStates; ++p) col[p] = (p == t) ? 1.0 : 0.0;
+      (void)chain_seg_cascade<double>(S.seg[k], col, 0.0);
+#pragma unroll
+      for (int p = 0; p < kChainStates; ++p) M[p][t] = col[p];
+    }
+    __syncthreads();
+    double* pw = W.pw + (long long)b * kWideLogT * kChainStates * kChainStates;
+    for (int s = 1; s <= kWideLogLc + kWideLogT; ++s) {
+      double a = 0.0;
+      if (t < kChainStates * kChainStates) {
+#pragma unroll
+        for (int p = 0; p < kChainStates; ++p) a = fma(M[q][p], M[p][r], a);
+      }
+      __syncthreads();
+      if (t < kChainStates * kChainStates) {
+        M[q][r] = a;
+        if (s >= kWideLogLc && s < kWideLogLc + kWideLogT) pw[(s - kWideLogLc) * kChainStates * kChainStates + t] = a;
+      }
+      __syncthreads();
+    }
+    for (int j = t; j < kSegStates * kSegStates; j += kWideT) {
+      const int p = j / kSegStates, c = j % kSegStates;
+      mb[j] = (p < kChainStates && c < kChainStates) ? M[p][c] : (p == c ? 1.0 : 0.0);
+    }
+    return;
+  }
+  const long long i0 = base + (long long)t * kWideLc;
+  const int m = chain_seg_len(n, i0);
+  double* tc = W.tc + ((long long)b * kWideT + t) * kSegStates * kSegStates;
+#pragma unroll 1
+  for (int j = 0; j < kSegStates; ++j) {
+    double col[kSegStates];
+    chain_seg_column(S, i0, m, j, col);
+#pragma unroll
+    for (int p = 0; p < kSegStates; ++p) tc[p * kSegStates + j] = col[p];
+  }
+  __syncthreads();
+  const double* T = W.tc + (long long)b * kWideT * kSegStates * kSegStates;
+  const int q = t / kSegStates, r = t % kSegStates;
+  const bool act = t < kSegStates * kSegStates;
+  if (act) M[q][r] = T[t];
+  __syncthreads();
+#pragma unroll 1
+  for (int c = 1; c < kWideT; ++c) {    // M <- T_c M
+    double a = 0.0;
+    if (act) {
+      const double* Tc = T + (long long)c * kSegStates * kSegStates + q * kSegStates;
+#pragma unroll
+      for (int p = 0; p < kSegStates; ++p) a = fma(Tc[p], M[p][r], a);
+    }
+    __syncthreads();
+    if (act) M[q][r] = a;
+    __syncthreads();
+  }
+  if (act) mb[t] = M[q][r];
+}
+
+// pass 1: zero-state end points and the CTA aggregate.  grid (CTAs, 2 channels)
+static __global__ void __launch_bounds__(kWideT) k_chain_seg_pass1(ChainSendParams P, ChainSegs S, ChainSegScratch W) {
+  __shared__ float buf[kWideT][kWideLc + 1];
+  __shared__ double V[kSegStates * kWideT];
+  __shared__ double PW[kWideLogT][kChainStates][kChainStates];
+  __shared__ double Sv[kSegStates];
+  const int ch = blockIdx.y, b = blockIdx.x, t = threadIdx.x;
+  const long long base = (long long)b * kWideSpan, end = base + kWideSpan < P.n ? base + kWideSpan : P.n;
+  const int k = chain_seg_uniform(S, base, end);
+  chain_wide_stage(P, ch, base, buf);
+  if (k >= 0)
+    for (int j = t; j < kWideLogT * kChainStates * kChainStates; j += kWideT)
+      (&PW[0][0][0])[j] = W.pw[(long long)b * kWideLogT * kChainStates * kChainStates + j];
+  if (t < kSegStates) Sv[t] = 0.0;
+  __syncthreads();
+  float s[kSegStates];
+#pragma unroll
+  for (int q = 0; q < kSegStates; ++q) s[q] = 0.0f;
+  const long long i0 = base + (long long)t * kWideLc;
+  chain_seg_run<float>(S, i0, chain_seg_len(P.n, i0), s, buf[t], nullptr);
+  float* z = W.z + (((long long)ch * W.nb_cap + b) * kWideT + t) * kSegStates;
+#pragma unroll
+  for (int q = 0; q < kSegStates; ++q) { z[q] = s[q]; V[q * kWideT + t] = s[q]; }
+  __syncthreads();
+  double* agg = W.agg + ((long long)ch * W.nb_cap + b) * kSegStates;
+  if (k >= 0) {                         // k_chain_wide_pass1's tree
+#pragma unroll 1
+    for (int j = 0, d = 1; d < kWideT; ++j, d *= 2) {
+      double nx[kChainStates];
+      const bool act = (t & (2 * d - 1)) == 0;
+      if (act) chain_combine(PW[j], V, kWideT, t, d, true, nx);
+      __syncthreads();
+      if (act) {
+#pragma unroll
+        for (int q = 0; q < kChainStates; ++q) V[q * kWideT + t] = nx[q];
+      }
+      __syncthreads();
+    }
+    if (t < kSegStates) agg[t] = t < kChainStates ? V[t * kWideT] : 0.0;
+  } else {
+    chain_seg_serial(W.tc + (long long)b * kWideT * kSegStates * kSegStates, V, Sv, false);
+    if (t < kSegStates) agg[t] = Sv[t];
+  }
+}
+
+// carry: G_0 = the carried state (scan slots and stash), G_{b+1} = M_b G_b + agg_b.  grid (2 channels), 32 threads
+static __global__ void __launch_bounds__(32) k_chain_seg_carry(ChainSendParams P, ChainSegScratch W, long long nb) {
+  __shared__ double G[kSegStates];
+  const int ch = blockIdx.x, q = threadIdx.x;
+  if (q < kSegStates) G[q] = P.state[ch * kChainStateStride + q];
+  __syncwarp();
+  double* out = W.carry + (long long)ch * W.nb_cap * kSegStates;
+  const double* agg = W.agg + (long long)ch * W.nb_cap * kSegStates;
+#pragma unroll 1
+  for (long long b = 0; b < nb; ++b) {
+    double a = 0.0;
+    if (q < kSegStates) {
+      out[b * kSegStates + q] = G[q];
+      a = agg[b * kSegStates + q];
+      const double* row = W.mb + (b * kSegStates + q) * kSegStates;
+#pragma unroll
+      for (int r = 0; r < kSegStates; ++r) a = fma(row[r], G[r], a);
+    }
+    __syncwarp();
+    if (q < kSegStates) G[q] = a;
+    __syncwarp();
+  }
+}
+
+// pass 2: every chunk's true initial state, the filtered chunks, the ring.  grid (CTAs, 2 channels)
+static __global__ void __launch_bounds__(kWideT) k_chain_seg_pass2(ChainSendParams P, ChainSegs S, ChainSegScratch W) {
+  __shared__ float buf[kWideT][kWideLc + 1];
+  __shared__ double V[kSegStates * kWideT];
+  __shared__ double PW[kWideLogT][kChainStates][kChainStates];
+  __shared__ double Sv[kSegStates];
+  const int ch = blockIdx.y, b = blockIdx.x, t = threadIdx.x;
+  const long long base = (long long)b * kWideSpan, end = base + kWideSpan < P.n ? base + kWideSpan : P.n;
+  const int k = chain_seg_uniform(S, base, end);
+  chain_wide_stage(P, ch, base, buf);
+  const double* g = W.carry + ((long long)ch * W.nb_cap + b) * kSegStates;
+  const float* z = W.z + (((long long)ch * W.nb_cap + b) * kWideT + t) * kSegStates;
+#pragma unroll
+  for (int q = 0; q < kSegStates; ++q) V[q * kWideT + t] = z[q];
+  if (t < kSegStates) Sv[t] = g[t];
+  float s[kSegStates];
+  if (k >= 0) {                         // k_chain_wide_pass2's seed and scan
+    for (int j = t; j < kWideLogT * kChainStates * kChainStates; j += kWideT)
+      (&PW[0][0][0])[j] = W.pw[(long long)b * kWideLogT * kChainStates * kChainStates + j];
+    __syncthreads();
+    double G[kChainStates] = {0, 0, 0, 0, 0, 0, 0, 0};
+    if (t == 0) {
+      double acc[kChainStates];
+#pragma unroll
+      for (int q = 0; q < kChainStates; ++q) { G[q] = Sv[q]; acc[q] = V[q * kWideT]; }
+      chain_affine_acc(PW[0], G, acc);
+#pragma unroll
+      for (int q = 0; q < kChainStates; ++q) V[q * kWideT] = acc[q];
+    }
+    __syncthreads();
+    chain_wide_scan<kWideT>(PW, V);
+#pragma unroll
+    for (int q = 0; q < kChainStates; ++q) s[q] = (float)(t == 0 ? G[q] : V[q * kWideT + t - 1]);
+    s[kChainStates] = (float)Sv[kChainStates];
+    s[kChainStates + 1] = (float)Sv[kChainStates + 1];
+  } else {
+    __syncthreads();
+    chain_seg_serial(W.tc + (long long)b * kWideT * kSegStates * kSegStates, V, Sv, true);
+#pragma unroll
+    for (int q = 0; q < kSegStates; ++q) s[q] = (float)V[q * kWideT + t];
+  }
+  const long long i0 = base + (long long)t * kWideLc;
+  const int m = chain_seg_len(P.n, i0);
+  chain_seg_run<float>(S, i0, m, s, buf[t], buf[t]);
+  if (m > 0 && i0 + m == P.n) {         // the state after the piece's last sample, stash included
+#pragma unroll
+    for (int q = 0; q < kSegStates; ++q) P.state[ch * kChainStateStride + q] = s[q];
+  }
+  __syncthreads();
+  for (int j = t; j < kWideSpan; j += kWideT) {
+    const long long i = base + j;
+    if (i < P.n) {
+      const float y = buf[j / kWideLc][j % kWideLc];
+      P.ring[(long long)ch * P.ring_stride + ((P.ring_pos + i) & P.ring_mask)] = y;
+      if (P.filt) P.filt[(long long)ch * P.filt_stride + i] = y;
+    }
+  }
+}
+
+// read: the predelayed convolver input per sample.  grid (blocks of 256 samples, 2 channels); the block finds its first
+// row once, each thread walks from there
+static __global__ void __launch_bounds__(256) k_chain_seg_read(ChainSendParams P, ChainSegs S) {
+  __shared__ int k0;
+  const long long base = (long long)blockIdx.x * blockDim.x, i = base + threadIdx.x;
+  if (threadIdx.x == 0) k0 = chain_seg_at(S, base);
+  __syncthreads();
+  if (i >= P.n) return;
+  int k = k0;
+  while (k + 1 < S.nseg && S.seg[k + 1].start <= S.off + i) ++k;
+  chain_seg_ring_read(P, S.seg[k], blockIdx.y, i);
+}
+
+// k_chain_wet with the row of each sample.  grid (blocks of 256 samples)
+static __global__ void __launch_bounds__(256) k_chain_wet_seg(ChainWetParams P, ChainSegs S) {
+  __shared__ int k0;
+  const long long base = (long long)blockIdx.x * blockDim.x, i = base + threadIdx.x;
+  if (threadIdx.x == 0) k0 = chain_seg_at(S, base);
+  __syncthreads();
+  if (i >= P.n) return;
+  int k = k0;
+  while (k + 1 < S.nseg && S.seg[k + 1].start <= S.off + i) ++k;
+  chain_wet_seg_sample(P, S.seg[k], i);
+}
 #else
 // CPU emulation (tests/emu): same chunking, same two passes
 inline void emu_chain_send(const ChainSendParams& P, int T) {
@@ -697,6 +1067,181 @@ inline void emu_chain_wide(const ChainSendParams& P, const ChainWideScratch& W, 
     }
   delete[] buf;
   delete[] V;
+}
+// the segmented form: the same maps, chunking, folds and scan order, one CTA / thread after another
+inline void emu_chain_seg_serial(const double* tc, double* V, double* Sv, bool seeds) {
+  for (int c = 0; c < kWideT; ++c) {
+    double a[kSegStates];
+    for (int q = 0; q < kSegStates; ++q) {
+      a[q] = V[q * kWideT + c];
+      if (seeds) V[q * kWideT + c] = Sv[q];
+      const double* row = tc + ((long long)c * kSegStates + q) * kSegStates;
+      for (int r = 0; r < kSegStates; ++r) a[q] = fma(row[r], Sv[r], a[q]);
+    }
+    for (int q = 0; q < kSegStates; ++q) Sv[q] = a[q];
+  }
+}
+inline void emu_chain_seg(const ChainSendParams& P, const ChainSegs& S, const ChainSegScratch& W) {
+  constexpr int S2 = kChainStates * kChainStates, T2 = kSegStates * kSegStates;
+  const long long nb = chain_wide_ctas(P.n);
+  auto cta_end = [&](long long base) { return base + kWideSpan < P.n ? base + kWideSpan : P.n; };
+  for (long long b = 0; b < nb; ++b) {             // maps
+    const long long base = b * kWideSpan;
+    const int k = chain_seg_uniform(S, base, cta_end(base));
+    double* mb = W.mb + b * T2;
+    if (k >= 0) {
+      double M[kChainStates][kChainStates], nx[kChainStates][kChainStates];
+      for (int j = 0; j < kChainStates; ++j) {
+        double col[kChainStates];
+        for (int p = 0; p < kChainStates; ++p) col[p] = (p == j) ? 1.0 : 0.0;
+        (void)chain_seg_cascade<double>(S.seg[k], col, 0.0);
+        for (int p = 0; p < kChainStates; ++p) M[p][j] = col[p];
+      }
+      for (int s = 1; s <= kWideLogLc + kWideLogT; ++s) {
+        for (int q = 0; q < kChainStates; ++q)
+          for (int r = 0; r < kChainStates; ++r) nx[q][r] = chain_square_entry(M, q, r);
+        for (int q = 0; q < kChainStates; ++q)
+          for (int r = 0; r < kChainStates; ++r) {
+            M[q][r] = nx[q][r];
+            if (s >= kWideLogLc && s < kWideLogLc + kWideLogT) W.pw[(b * kWideLogT + s - kWideLogLc) * S2 + q * kChainStates + r] = nx[q][r];
+          }
+      }
+      for (int p = 0; p < kSegStates; ++p)
+        for (int c = 0; c < kSegStates; ++c)
+          mb[p * kSegStates + c] = (p < kChainStates && c < kChainStates) ? M[p][c] : (p == c ? 1.0 : 0.0);
+      continue;
+    }
+    const double* T = W.tc + b * kWideT * T2;
+    for (int t = 0; t < kWideT; ++t) {
+      const long long i0 = base + (long long)t * kWideLc;
+      double* tc = W.tc + (b * kWideT + t) * T2;
+      for (int j = 0; j < kSegStates; ++j) {
+        double col[kSegStates];
+        chain_seg_column(S, i0, chain_seg_len(P.n, i0), j, col);
+        for (int p = 0; p < kSegStates; ++p) tc[p * kSegStates + j] = col[p];
+      }
+    }
+    double M[kSegStates][kSegStates], nx[kSegStates][kSegStates];
+    for (int j = 0; j < T2; ++j) M[j / kSegStates][j % kSegStates] = T[j];
+    for (int c = 1; c < kWideT; ++c) {
+      for (int q = 0; q < kSegStates; ++q)
+        for (int r = 0; r < kSegStates; ++r) {
+          double a = 0.0;
+          for (int p = 0; p < kSegStates; ++p) a = fma(T[c * T2 + q * kSegStates + p], M[p][r], a);
+          nx[q][r] = a;
+        }
+      std::memcpy(M, nx, sizeof(M));
+    }
+    for (int j = 0; j < T2; ++j) mb[j] = M[j / kSegStates][j % kSegStates];
+  }
+  float (*buf)[kWideLc + 1] = new float[kWideT][kWideLc + 1];
+  double* V = new double[(size_t)kSegStates * kWideT];
+  const double (*PWall)[kChainStates][kChainStates] = reinterpret_cast<const double (*)[kChainStates][kChainStates]>(W.pw);
+  auto stage = [&](int ch, long long base) {
+    for (int j = 0; j < kWideSpan; ++j) {
+      const long long i = base + j;
+      buf[j / kWideLc][j % kWideLc] = i < P.n ? chain_wide_send(P, ch, i) : 0.0f;
+    }
+  };
+  for (int ch = 0; ch < 2; ++ch)                   // pass 1
+    for (long long b = 0; b < nb; ++b) {
+      const long long base = b * kWideSpan;
+      const int k = chain_seg_uniform(S, base, cta_end(base));
+      stage(ch, base);
+      for (int t = 0; t < kWideT; ++t) {
+        float s[kSegStates] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+        const long long i0 = base + (long long)t * kWideLc;
+        chain_seg_run<float>(S, i0, chain_seg_len(P.n, i0), s, buf[t], nullptr);
+        float* z = W.z + (((long long)ch * W.nb_cap + b) * kWideT + t) * kSegStates;
+        for (int q = 0; q < kSegStates; ++q) { z[q] = s[q]; V[q * kWideT + t] = s[q]; }
+      }
+      double* agg = W.agg + ((long long)ch * W.nb_cap + b) * kSegStates;
+      if (k >= 0) {
+        const double (*PW)[kChainStates][kChainStates] = PWall + b * kWideLogT;
+        for (int j = 0, d = 1; d < kWideT; ++j, d *= 2)
+          for (int t = 0; t < kWideT; t += 2 * d) {
+            double nx[kChainStates];
+            chain_combine(PW[j], V, kWideT, t, d, true, nx);
+            for (int q = 0; q < kChainStates; ++q) V[q * kWideT + t] = nx[q];
+          }
+        for (int q = 0; q < kSegStates; ++q) agg[q] = q < kChainStates ? V[q * kWideT] : 0.0;
+      } else {
+        double Sv[kSegStates] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+        emu_chain_seg_serial(W.tc + b * kWideT * T2, V, Sv, false);
+        for (int q = 0; q < kSegStates; ++q) agg[q] = Sv[q];
+      }
+    }
+  for (int ch = 0; ch < 2; ++ch) {                 // carry
+    double G[kSegStates];
+    for (int q = 0; q < kSegStates; ++q) G[q] = P.state[ch * kChainStateStride + q];
+    double* out = W.carry + (long long)ch * W.nb_cap * kSegStates;
+    const double* agg = W.agg + (long long)ch * W.nb_cap * kSegStates;
+    for (long long b = 0; b < nb; ++b) {
+      double a[kSegStates];
+      for (int q = 0; q < kSegStates; ++q) {
+        out[b * kSegStates + q] = G[q];
+        a[q] = agg[b * kSegStates + q];
+        for (int r = 0; r < kSegStates; ++r) a[q] = fma(W.mb[(b * kSegStates + q) * kSegStates + r], G[r], a[q]);
+      }
+      for (int q = 0; q < kSegStates; ++q) G[q] = a[q];
+    }
+  }
+  for (int ch = 0; ch < 2; ++ch)                   // pass 2
+    for (long long b = 0; b < nb; ++b) {
+      const long long base = b * kWideSpan;
+      const int k = chain_seg_uniform(S, base, cta_end(base));
+      stage(ch, base);
+      const double* g = W.carry + ((long long)ch * W.nb_cap + b) * kSegStates;
+      for (int t = 0; t < kWideT; ++t) {
+        const float* z = W.z + (((long long)ch * W.nb_cap + b) * kWideT + t) * kSegStates;
+        for (int q = 0; q < kSegStates; ++q) V[q * kWideT + t] = z[q];
+      }
+      double G[kChainStates];
+      if (k >= 0) {
+        const double (*PW)[kChainStates][kChainStates] = PWall + b * kWideLogT;
+        double acc[kChainStates];
+        for (int q = 0; q < kChainStates; ++q) { G[q] = g[q]; acc[q] = V[q * kWideT]; }
+        chain_affine_acc(PW[0], G, acc);
+        for (int q = 0; q < kChainStates; ++q) V[q * kWideT] = acc[q];
+        emu_chain_wide_scan(PW, V, kWideT);
+      } else {
+        double Sv[kSegStates];
+        for (int q = 0; q < kSegStates; ++q) Sv[q] = g[q];
+        emu_chain_seg_serial(W.tc + b * kWideT * T2, V, Sv, true);
+      }
+      for (int t = 0; t < kWideT; ++t) {
+        float s[kSegStates];
+        if (k >= 0) {
+          for (int q = 0; q < kChainStates; ++q) s[q] = (float)(t == 0 ? G[q] : V[q * kWideT + t - 1]);
+          s[kChainStates] = (float)g[kChainStates];
+          s[kChainStates + 1] = (float)g[kChainStates + 1];
+        } else {
+          for (int q = 0; q < kSegStates; ++q) s[q] = (float)V[q * kWideT + t];
+        }
+        const long long i0 = base + (long long)t * kWideLc;
+        const int m = chain_seg_len(P.n, i0);
+        chain_seg_run<float>(S, i0, m, s, buf[t], buf[t]);
+        if (m > 0 && i0 + m == P.n)
+          for (int q = 0; q < kSegStates; ++q) P.state[ch * kChainStateStride + q] = s[q];
+      }
+      for (int j = 0; j < kWideSpan; ++j) {
+        const long long i = base + j;
+        if (i < P.n) {
+          const float y = buf[j / kWideLc][j % kWideLc];
+          P.ring[(long long)ch * P.ring_stride + ((P.ring_pos + i) & P.ring_mask)] = y;
+          if (P.filt) P.filt[(long long)ch * P.filt_stride + i] = y;
+        }
+      }
+    }
+  delete[] buf;
+  delete[] V;
+}
+inline void emu_chain_seg_read(const ChainSendParams& P, const ChainSegs& S) {
+  for (int ch = 0; ch < 2; ++ch)
+    for (long long i = 0; i < P.n; ++i) chain_seg_ring_read(P, S.seg[chain_seg_at(S, i)], ch, i);
+}
+inline void emu_chain_wet_seg(const ChainWetParams& P, const ChainSegs& S) {
+  for (long long i = 0; i < P.n; ++i) chain_wet_seg_sample(P, S.seg[chain_seg_at(S, i)], i);
 }
 inline void emu_chain_wet(const ChainWetParams& P) {
   for (long long i = 0; i < P.n; ++i) chain_wet_sample(P, i);
