@@ -127,6 +127,37 @@ size_t b200conv_latency(const b200conv_t* h);
 /* calls in fixed-latency mode that had to wait for device work (the host's underrun indicator); reset by set_latency */
 unsigned long long b200conv_latency_waits(const b200conv_t* h);
 
+/* Groups of handles (beyond the reference): the real-time calls of several handles in one launch, for hosts that drive
+ * several instances from one audio callback (a session with several reverbs, one handle per zone of a game engine).
+ * Semantics: b200conv_group_process(g, in, out, len) is exactly b200conv_process(members[i], in[i], out[i], len) for
+ * every i, in member order; outputs and handle states are what those calls would leave, within float rounding.
+ * A member QUALIFIES for a call when b200conv_process would run it as one cluster launch (a call of at most one head
+ * block on a head stage that fits one cluster) and it is unsharded, not in fixed-latency mode, timing is off and it has
+ * zero-copy staging and a completion word.  Qualifying members with the same head block, channel count and cluster
+ * width form one shape class: one launch per class (per 32 members), one cluster per member; routing / mixdown, the
+ * stages and whether the call crosses a head-block boundary may differ inside a class.  Every other member (split-mode
+ * uniform long IRs, C > 8, len above the head block, a latency handle, timing on, a tail shard, no IR, ...) runs its
+ * ordinary b200conv_process inside the group call, after the shared launches are enqueued.  The host waits once per
+ * call for all shared launches.
+ * Errors: b200conv_group_create returns NULL for n < 1, n > 64, a NULL or repeated member, members on different
+ * devices, or when it runs out of memory or CUDA resources.  b200conv_group_process checks every member's arguments
+ * (in / out / in[i] / out[i] NULL with len > 0, as b200conv_process does) before it enqueues anything: B200CONV_EINVAL
+ * (B200CONV_ECUDA for a member whose CUDA context failed) and no member advances.  len == 0 does nothing.  A CUDA error
+ * inside the call returns the first error; members already processed stay processed.
+ * Lifetime / threading: members must outlive the group; while a group call runs no other thread may call a member.
+ * Between group calls the members stay fully usable on their own (device calls, clear, reset, init_* included).
+ * Steady state: a group call allocates nothing, never synchronises, makes one driver launch per shape class and no
+ * event operation unless a member completes a tail block or has unsynchronised work queued on its own stream. */
+typedef struct b200conv_group b200conv_group_t;
+b200conv_group_t*  b200conv_group_create(b200conv_t* const* members, int n);
+void               b200conv_group_destroy(b200conv_group_t* g);
+const char*        b200conv_group_last_error(const b200conv_group_t* g);
+/* in[i] / out[i]: what b200conv_process(members[i], in[i], out[i], len) takes */
+int                b200conv_group_process(b200conv_group_t* g, const float* const* const* in,
+                                          float* const* const* out, size_t len);
+/* cluster launches of the group's shared calls (members count only the tail blocks they enqueue) */
+unsigned long long b200conv_group_launch_count(const b200conv_group_t* g);
+
 /* Introspection --------------------------------------------------------------------------- */
 typedef struct b200conv_stage_info {
   size_t block;        /* B_s                                  */

@@ -394,6 +394,62 @@ class Engine:
             pass
 
 
+class Group:
+    """Several Engines whose real-time calls run together (b200conv_group_process): process(inputs) is
+    engines[i].process(inputs[i]) for every i, with the calls that fit one cluster launch sharing one launch per
+    shape class.  Keeps references to its engines, which must stay open while the group is."""
+
+    def __init__(self, engines: Sequence[Engine], lib=None):
+        self._l = lib or engines[0]._l
+        self.engines = list(engines)
+        hs = (C.c_void_p * len(self.engines))(*[e._h for e in self.engines])
+        self._g = self._l.b200conv_group_create(hs, len(self.engines))
+        if not self._g:
+            raise B200ConvError("b200conv_group_create failed")
+
+    def process(self, inputs) -> list:
+        """inputs[i]: what engines[i].process takes (equally long calls); returns the list of their outputs."""
+        xs = [[np.ascontiguousarray(a, dtype=np.float32) for a in x] for x in inputs]
+        if len(xs) != len(self.engines):
+            raise ValueError("need one input list per engine")
+        n = xs[0][0].size
+        ys, ins, outs = [], (C.c_void_p * len(xs))(), (C.c_void_p * len(xs))()
+        keep = []
+        for i, (e, x) in enumerate(zip(self.engines, xs)):
+            n_in = getattr(e, "_n_in", None) or e.n_channels
+            n_out = getattr(e, "_n_out", None) or e.n_channels
+            if len(x) != n_in or any(a.size != n for a in x):
+                raise ValueError("need one equally long input per (routed) input channel of every engine")
+            y = [np.empty(max(n, 1), np.float32)[:n] for _ in range(n_out)]
+            pi, po = _ptr_array(x), _ptr_array(y)
+            keep += [pi, po]
+            ins[i], outs[i] = C.cast(pi, C.c_void_p), C.cast(po, C.c_void_p)
+            ys.append(y)
+        if n:
+            self._check(self._l.b200conv_group_process(self._g, C.cast(ins, C.POINTER(C.c_void_p)),
+                                                       C.cast(outs, C.POINTER(C.c_void_p)), n))
+        return ys
+
+    def _check(self, rc: int) -> None:
+        if rc != 0:
+            raise B200ConvError(f"group process failed ({rc}): {self._l.b200conv_group_last_error(self._g).decode()}")
+
+    @property
+    def launch_count(self) -> int:
+        return int(self._l.b200conv_group_launch_count(self._g))
+
+    def close(self):
+        if getattr(self, "_g", None):
+            self._l.b200conv_group_destroy(self._g)
+            self._g = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def ir_decay_eq(ir, lut, srate: float, device: int = 0, lib=None) -> np.ndarray:
     """Device version of Impulse::applyDecay (src/dsp/Impulse.cpp:602-648): returns the shaped IR."""
     lib = lib or _lib.default()

@@ -258,6 +258,11 @@ struct b200conv {
   LatRing* lat = nullptr;                   // b200conv_process: C rows each way (routing uses n_in / n_out of them)
   LatRing* c_lat = nullptr;                 // b200conv_chain_process: dry L, dry R, ysend, yrev in; L, R out (moves with the chain)
   unsigned long long lat_waits = 0;         // waits for a step that had not completed (since set_latency)
+  // groups (b200conv_group_process): s_main may hold work the host has not seen complete (every entry point sets it in
+  // set_device, a real-time call that saw its completion word clears it); a group's event this handle's next own call
+  // orders s_main and s_post behind (nullptr: none)
+  bool main_unsynced = false;
+  cudaEvent_t grp_ev = nullptr;
 };
 
 namespace {
@@ -1037,8 +1042,17 @@ int launch_cmac_exchange(b200conv* h, const pc::CmacParams& P, int C, const Tail
   return resident ? launch_cmac_stream_tma(h, P, C, 12, 1, false, -1.0f, &x) : launch_cmac_stream_tma(h, P, C, 6, 2, false, -1.0f, &x);
 }
 
+// First thing of every entry point that enqueues device work.  After a group call that recorded its event this
+// handle's streams are ordered behind the group's shared launch and the tail-output waits it queued (the lazy wait of
+// b200conv_group_process).
 int set_device(b200conv* h) {
   CU_CHECK(h, cudaSetDevice(h->cfg.device));
+  h->main_unsynced = true;
+  if (h->grp_ev) {
+    CU_CHECK(h, cudaStreamWaitEvent(h->s_main, h->grp_ev, 0));
+    CU_CHECK(h, cudaStreamWaitEvent(h->s_post, h->grp_ev, 0));
+    h->grp_ev = nullptr;
+  }
   return 0;
 }
 
@@ -2032,8 +2046,9 @@ int rt_cluster_ctas(const b200conv* h, size_t len) {
 }
 
 #if !defined(PC_EMULATE)
-template <int M>
-cudaError_t rt_launch_m(const pc::RtParams& P, int nctas, size_t smem, cudaStream_t st) {
+// grid of `nctas` CTAs in clusters of `cluster`
+template <class Arg>
+cudaError_t rt_launch_kernel(void (*k)(Arg), const Arg& a, int nctas, int cluster, size_t smem, cudaStream_t st) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(nctas, 1, 1);
   cfg.blockDim = dim3(256, 1, 1);
@@ -2041,22 +2056,49 @@ cudaError_t rt_launch_m(const pc::RtParams& P, int nctas, size_t smem, cudaStrea
   cfg.stream = st;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = nctas; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+  at[0].val.clusterDim.x = cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg.attrs = at; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, pc::k_rt_block<M>, P);
+  return cudaLaunchKernelEx(&cfg, k, a);
+}
+template <int M>
+cudaError_t rt_launch_m(const pc::RtParams& P, int cluster, size_t smem, cudaStream_t st) {
+  return rt_launch_kernel(pc::k_rt_block<M>, P, cluster, cluster, smem, st);
+}
+template <int M>
+cudaError_t rt_launch_m(const pc::RtGroupParams& G, int cluster, size_t smem, cudaStream_t st) {
+  return rt_launch_kernel(pc::k_rt_group<M>, G, G.n * cluster, cluster, smem, st);
+}
+// k_rt_block<M> (one call) or k_rt_group<M> (a group's shape class) with clusters of C * NC CTAs
+template <class Arg>
+cudaError_t rt_launch(const Arg& a, int M, int C, int NC, cudaStream_t st) {
+  const size_t smem = (size_t)pc::rt_smem_layout(M, C).bytes;
+  switch (M) {
+    case 16: return rt_launch_m<16>(a, C * NC, smem, st);
+    case 32: return rt_launch_m<32>(a, C * NC, smem, st);
+    case 64: return rt_launch_m<64>(a, C * NC, smem, st);
+    case 128: return rt_launch_m<128>(a, C * NC, smem, st);
+    case 256: return rt_launch_m<256>(a, C * NC, smem, st);
+    case 512: return rt_launch_m<512>(a, C * NC, smem, st);
+    case 1024: return rt_launch_m<1024>(a, C * NC, smem, st);
+    default: return cudaErrorInvalidValue;
+  }
 }
 template <int M>
 bool rt_set_attr() {
   const int smem = pc::rt_smem_layout(M, 16).bytes;
   return cudaFuncSetAttribute(pc::k_rt_block<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
-         cudaFuncSetAttribute(pc::k_rt_block<M>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
+         cudaFuncSetAttribute(pc::k_rt_block<M>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess &&
+         cudaFuncSetAttribute(pc::k_rt_group<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
+         cudaFuncSetAttribute(pc::k_rt_group<M>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
 }
 #endif
 
-// One real-time call (rt_cluster_ctas() > 0): `in` / `out` are device-accessible (pinned host or device memory).
-// done_flag (device address of a pinned word, or nullptr): raised to done_val once every output sample is written.
-int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, size_t out_stride, size_t len,
-            unsigned int* done_flag, unsigned int done_val) {
+// A real-time call (rt_cluster_ctas() > 0) runs as prepare, launch, commit; b200conv_group_process prepares several
+// handles, launches them together and commits them.  `in` / `out` are device-accessible (pinned host or device memory).
+// Prepare: the waits for tail outputs the call needs (queued on `st`, the stream the launch goes to; *waited is set if
+// there was one), room in the timeline, and the call's parameters.  Split mode (nc < 0) is set up by rt_call.
+int rt_prepare(b200conv* h, int nc, const float* in, size_t in_stride, float* out, size_t out_stride, size_t len,
+               cudaStream_t st, pc::RtParams& P, bool* waited) {
   const int C = h->C;
   Stage& s0 = h->stages[0];
   const int M = s0.B;
@@ -2065,15 +2107,16 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
     Stage& s = h->stages[si];
     for (int j = 0; j < 2; ++j)
       if (!s.job_waited[j] && h->abs_pos + (long long)len > s.job_out_start[j]) {
-        CU_CHECK(h, cudaStreamWaitEvent(h->s_main, s.ev_job[j], 0));
+        CU_CHECK(h, cudaStreamWaitEvent(st, s.ev_job[j], 0));
         s.job_waited[j] = true;
         h->rt_tail_joined = true;
+        *waited = true;
       }
   }
   // a call that crosses the block boundary: len1 samples complete the open block, the other r start the next one
   const int len1 = std::min((int)len, M - s0.fill), r = (int)len - len1;
   if (int rc = ensure_rows(h, s0, r ? 2 : 1)) return rc;
-  pc::RtParams P{};
+  P = pc::RtParams{};
   P.M = M; P.C = C; P.NC = nc; P.P = s0.P;
   P.len = (int)len; P.nseg = r ? 2 : 1;
   pc::RtSeg& S1 = P.seg[0];
@@ -2103,9 +2146,10 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
     // call ends after the boundary.  Deeper stages of b200conv_init_stages wait here.
     const int jp = (int)((s.njobs + 1) & 1);
     if (at_boundary && s.njobs && !s.job_waited[jp]) {
-      CU_CHECK(h, cudaStreamWaitEvent(h->s_main, s.ev_job[jp], 0));
+      CU_CHECK(h, cudaStreamWaitEvent(st, s.ev_job[jp], 0));
       s.job_waited[jp] = true;
       h->rt_tail_joined = true;
+      *waited = true;
     }
     P.add[na] = s.fut; P.add_cstride[na] = (long long)s.ring; P.add_mask[na] = (long long)s.ring - 1;
     ++na;
@@ -2114,57 +2158,25 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
   P.out = out; P.out_stride = (long long)out_stride;
   P.mix_on = h->route_on ? 1 : 0; P.n_out = h->route_on ? h->n_out : C;
   std::memcpy(P.mix, h->mix, sizeof(P.mix));
-  const bool split = nc < 0;
-  if (split) nc = 1;
-  P.NC = nc;
-  auto launch = [&](const pc::RtParams& Q) -> int {
-#if defined(PC_EMULATE)
-    pc::emu_rt_block(Q);
-#else
-    const size_t smem = (size_t)pc::rt_smem_layout(M, C).bytes;
-    cudaError_t e = cudaErrorInvalidValue;
-    switch (M) {
-      case 16: e = rt_launch_m<16>(Q, C * nc, smem, h->s_main); break;
-      case 32: e = rt_launch_m<32>(Q, C * nc, smem, h->s_main); break;
-      case 64: e = rt_launch_m<64>(Q, C * nc, smem, h->s_main); break;
-      case 128: e = rt_launch_m<128>(Q, C * nc, smem, h->s_main); break;
-      case 256: e = rt_launch_m<256>(Q, C * nc, smem, h->s_main); break;
-      case 512: e = rt_launch_m<512>(Q, C * nc, smem, h->s_main); break;
-      case 1024: e = rt_launch_m<1024>(Q, C * nc, smem, h->s_main); break;
-      default: break;
-    }
-    CU_CHECK(h, e);
-#endif
-    h->launches++;
-    return 0;
-  };
-  if (!split) {
-    P.done_flag = done_flag; P.done_val = done_val;
-    if (int rc = launch(P)) return rc;
-  } else {
-    // head stage too large for one cluster: FRONT (assemble + forward FFT + timeline row), the TMA streaming sweep
-    // over all SMs into Y row 1, BACK (overlap-add + inverse FFT + output) — still zero-copy I/O and no D2H/H2D
-    float2* Yb = s0.Y[s0.ybuf];
-    const size_t row = (size_t)C * M;
-    P.mode = 1;
-    if (int rc = launch(P)) return rc;
-    if (int rc = launch_cmac(h, sweep_params(s0, C, Yb, 1), C)) return rc;
-    P.mode = 2; P.Yt = Yb + row;
-    P.done_flag = done_flag; P.done_val = done_val;
-    if (int rc = launch(P)) return rc;
-  }
+  return 0;
+}
+
+// Commit: the bookkeeping of a launched call and the tail blocks it completes.  They go to the low-priority stream
+// behind event `ev`, which is recorded on `st` (behind the call's launch) by the first of them unless *recorded.
+int rt_commit(b200conv* h, const pc::RtParams& P, cudaEvent_t ev, cudaStream_t st, bool* recorded) {
+  Stage& s0 = h->stages[0];
+  const int len1 = P.seg[0].len, r = P.len - len1;
   // bookkeeping of the head stage
-  if (S1.complete) { s0.head += 1; s0.blocks_done += 1; s0.fill = r; s0.ybuf ^= 1; }
-  else s0.fill += (int)len;
-  h->abs_pos += (long long)len;
+  if (P.seg[0].complete) { s0.head += 1; s0.blocks_done += 1; s0.fill = r; s0.ybuf ^= 1; }
+  else s0.fill += P.len;
+  h->abs_pos += (long long)P.len;
   // later stages: the kernel appended the samples; a completed block goes to the low-priority stream
-  bool recorded = false;
   for (size_t si = 1; si < h->stages.size(); ++si) {
     Stage& s = h->stages[si];
     s.fill += len1;
     if (s.fill < s.B) { s.fill += r; continue; }
-    if (!recorded) { CU_CHECK(h, cudaEventRecord(h->ev_rt, h->s_main)); recorded = true; }
-    CU_CHECK(h, cudaStreamWaitEvent(h->s_tail, h->ev_rt, 0));
+    if (!*recorded) { CU_CHECK(h, cudaEventRecord(ev, st)); *recorded = true; }
+    CU_CHECK(h, cudaStreamWaitEvent(h->s_tail, ev, 0));
     const int j = (int)(s.njobs & 1);
     s.job_out_start[j] = (s.blocks_done + s.q) * (long long)s.B;
     h->s_launch = h->s_tail;
@@ -2178,6 +2190,45 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
     s.fill = r;                                   // ... which holds the samples after the boundary
   }
   return 0;
+}
+
+// one launch of the cluster kernel on s_main
+int rt_launch_one(b200conv* h, const pc::RtParams& P) {
+#if defined(PC_EMULATE)
+  pc::emu_rt_block(P);
+#else
+  CU_CHECK(h, rt_launch(P, P.M, P.C, P.NC, h->s_main));
+#endif
+  h->launches++;
+  return 0;
+}
+
+// One real-time call of one handle on its s_main.  done_flag (device address of a pinned word, or nullptr): raised to
+// done_val once every output sample is written.
+int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, size_t out_stride, size_t len,
+            unsigned int* done_flag, unsigned int done_val) {
+  const bool split = nc < 0;
+  pc::RtParams P;
+  bool waited = false;
+  if (int rc = rt_prepare(h, split ? 1 : nc, in, in_stride, out, out_stride, len, h->s_main, P, &waited)) return rc;
+  if (!split) {
+    P.done_flag = done_flag; P.done_val = done_val;
+    if (int rc = rt_launch_one(h, P)) return rc;
+  } else {
+    // head stage too large for one cluster: FRONT (assemble + forward FFT + timeline row), the TMA streaming sweep
+    // over all SMs into Y row 1, BACK (overlap-add + inverse FFT + output) — still zero-copy I/O and no D2H/H2D
+    Stage& s0 = h->stages[0];
+    float2* Yb = s0.Y[s0.ybuf];
+    const size_t row = (size_t)h->C * s0.B;
+    P.mode = 1;
+    if (int rc = rt_launch_one(h, P)) return rc;
+    if (int rc = launch_cmac(h, sweep_params(s0, h->C, Yb, 1), h->C)) return rc;
+    P.mode = 2; P.Yt = Yb + row;
+    P.done_flag = done_flag; P.done_val = done_val;
+    if (int rc = rt_launch_one(h, P)) return rc;
+  }
+  bool recorded = false;
+  return rt_commit(h, P, h->ev_rt, h->s_main, &recorded);
 }
 
 // b200conv_reset / b200conv_destroy of either handle of a pending IR hot swap: the live handle continues alone
@@ -2539,6 +2590,7 @@ static int process_impl(b200conv_t* h, const float* const* in, float* const* out
               std::chrono::steady_clock::now() - t0 > std::chrono::milliseconds(20)) break;
       }
       if (!done) CU_CHECK(h, cudaStreamSynchronize(h->s_main));
+      h->main_unsynced = false;           // the kernel was the last work on s_main
       if (out)
         for (int c = 0; c < Cout; ++c) std::memcpy(out[c], h->hpin_out + (size_t)c * len, len * sizeof(float));
       if (h->p2p_tail && h->rt_tail_joined) {     // a tail block's barrier has run: did it give up on a peer?
@@ -2721,6 +2773,206 @@ int b200conv_process(b200conv_t* h, const float* const* in, float* const* out, s
 int b200conv_prime(b200conv_t* h, const float* const* in, size_t len) {
   if (h && h->lat_D) return fail(h, B200CONV_ESTATE, "b200conv_prime is not available in fixed-latency mode");
   return process_impl(h, in, nullptr, len);
+}
+
+// ---- groups (b200conv_group_process) ---------------------------------------------------------------------------------
+// The real-time calls of the qualifying members run as one k_rt_group launch per shape class on the group's own
+// high-priority stream: prepare every member, launch, commit every member.  Event rules:
+//  - a member's tail-output waits (rt_prepare) go on the group stream;
+//  - a member whose s_main may hold unsynchronised work (main_unsynced) orders the group stream behind it once;
+//  - if either happened, or a member completes a tail block, the group records ONE event after its launches: the
+//    s_tail of every member that completes a tail block waits on it before run_tail_block, and every prepared member
+//    keeps it in grp_ev, so that its next own call orders s_main and s_post behind it (set_device).
+// A Stage's job_waited therefore means "ordered before this handle's next head-stage work", through s_main or through
+// the group stream and grp_ev.  In steady state (no tail block completes, nothing unsynchronised) a group call makes
+// no event operation at all: one launch per shape class, then one spin per member on its completion word.
+struct b200conv_group {
+  std::vector<b200conv*> m;
+  int device = 0;
+  std::string err;
+  cudaStream_t st = nullptr;
+  cudaEvent_t ev = nullptr;
+  unsigned long long launches = 0;
+  // per-call scratch, sized by create: a group call allocates nothing
+  std::vector<pc::RtParams> P;
+  std::vector<int> nc;                   // cluster width of a qualifying member, 0: it runs its own b200conv_process
+  std::vector<char> prepared, launched;
+  pc::RtGroupParams G;
+};
+
+static int group_fail(b200conv_group* g, int code, const std::string& msg) { g->err = msg; return code; }
+static int group_member_fail(b200conv_group* g, size_t i, int code) {
+  g->err = "member " + std::to_string(i) + ": " + g->m[i]->err;
+  return code;
+}
+
+// cluster width of a member's call when it can share the group's launch, else 0
+static int group_ctas(const b200conv* h, size_t len) {
+  if (h->cfg.shard_count != 1 || h->lat_D || h->stages.empty() || len > h->hpin_cap || !h->hpin_in_dev ||
+      !h->hpin_out_dev || !h->hflag_dev)
+    return 0;
+  return std::max(rt_cluster_ctas(h, len), 0);
+}
+
+b200conv_group_t* b200conv_group_create(b200conv_t* const* members, int n) {
+  if (!members || n < 1 || n > 64) return nullptr;
+  for (int i = 0; i < n; ++i) {
+    if (!members[i] || members[i]->cfg.device != members[0]->cfg.device) return nullptr;
+    for (int j = 0; j < i; ++j)
+      if (members[j] == members[i]) return nullptr;
+  }
+  b200conv_group* g = new (std::nothrow) b200conv_group();
+  if (!g) return nullptr;
+  try {
+    g->m.assign(members, members + n);
+    g->P.resize(n); g->nc.resize(n); g->prepared.resize(n); g->launched.resize(n);
+  } catch (...) {
+    delete g;
+    return nullptr;
+  }
+  g->device = members[0]->cfg.device;
+  int lo = 0, hi = 0;
+  bool ok = cudaSetDevice(g->device) == cudaSuccess && cudaDeviceGetStreamPriorityRange(&lo, &hi) == cudaSuccess;
+  ok = ok && cudaStreamCreateWithPriority(&g->st, cudaStreamNonBlocking, hi) == cudaSuccess;
+  ok = ok && cudaEventCreateWithFlags(&g->ev, cudaEventDisableTiming) == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    b200conv_group_destroy(g);
+    return nullptr;
+  }
+  return g;
+}
+
+void b200conv_group_destroy(b200conv_group_t* g) {
+  if (!g) return;
+  cudaSetDevice(g->device);
+  if (g->st) cudaStreamSynchronize(g->st);
+  for (b200conv* h : g->m)
+    if (h->grp_ev == g->ev) h->grp_ev = nullptr;        // everything the event covers has completed
+  if (g->ev) cudaEventDestroy(g->ev);
+  if (g->st) cudaStreamDestroy(g->st);
+  delete g;
+}
+
+const char* b200conv_group_last_error(const b200conv_group_t* g) { return g ? g->err.c_str() : "null group"; }
+
+unsigned long long b200conv_group_launch_count(const b200conv_group_t* g) { return g ? g->launches : 0; }
+
+int b200conv_group_process(b200conv_group_t* g, const float* const* const* in, float* const* const* out, size_t len) {
+  if (!g) return B200CONV_EINVAL;
+  if (len == 0) return B200CONV_OK;
+  if (!in || !out) return group_fail(g, B200CONV_EINVAL, "null buffer");
+  const size_t n = g->m.size();
+  // every member's arguments before anything is enqueued: a refused call advances no member
+  for (size_t i = 0; i < n; ++i) {
+    const b200conv* h = g->m[i];
+    if (h->sticky_cuda_error) return group_member_fail(g, i, B200CONV_ECUDA);
+    if (!in[i] || !out[i]) return group_fail(g, B200CONV_EINVAL, "null buffer of member " + std::to_string(i));
+    if (h->lat_D)
+      for (int c = 0; c < (h->route_on ? h->n_in : h->C); ++c)
+        if (!in[i][c]) return group_fail(g, B200CONV_EINVAL, "null buffer of member " + std::to_string(i));
+  }
+  if (cudaSetDevice(g->device) != cudaSuccess) {
+    cudaGetLastError();
+    return group_fail(g, B200CONV_ECUDA, "cudaSetDevice failed");
+  }
+  int rc = 0;
+  bool waited = false;
+  // prepare: inputs into the pinned staging, the waits each call needs, its parameters
+  for (size_t i = 0; i < n; ++i) {
+    b200conv* h = g->m[i];
+    g->prepared[i] = g->launched[i] = 0;
+    g->nc[i] = group_ctas(h, len);
+    if (!g->nc[i] || rc) continue;
+    if (h->main_unsynced) {
+      cudaError_t e = cudaEventRecord(h->ev_rt, h->s_main);
+      if (e == cudaSuccess) e = cudaStreamWaitEvent(g->st, h->ev_rt, 0);
+      if (e != cudaSuccess) {
+        rc = group_member_fail(g, i, cuda_fail(h, e, "group: ordering behind the member's stream"));
+        continue;
+      }
+      h->main_unsynced = false;
+      waited = true;
+    }
+    const int Cin = h->route_on ? h->n_in : h->C;
+    for (int c = 0; c < Cin; ++c) std::memcpy(h->hpin_in + (size_t)c * len, in[i][c], len * sizeof(float));
+    h->s_launch = g->st;                   // a timeline compaction goes to the group stream, ahead of the launch
+    const int prc = rt_prepare(h, g->nc[i], h->hpin_in_dev, len, h->hpin_out_dev, len, len, g->st, g->P[i], &waited);
+    h->s_launch = h->s_main;
+    g->prepared[i] = 1;                    // waits may have been queued even if it failed
+    if (prc) { rc = group_member_fail(g, i, prc); continue; }
+    g->P[i].done_flag = h->hflag_dev;
+    g->P[i].done_val = ++h->flag_epoch;
+  }
+  // launch: one per shape class (M, C, NC) and kRtGroupMax members, in member order within a class
+  for (size_t i = 0; i < n && !rc; ++i) {
+    if (!g->prepared[i] || g->launched[i]) continue;
+    const pc::RtParams& A = g->P[i];
+    size_t idx[pc::kRtGroupMax];
+    int k = 0;
+    for (size_t j = i; j < n && k < pc::kRtGroupMax; ++j) {
+      const pc::RtParams& B = g->P[j];
+      if (g->prepared[j] && !g->launched[j] && B.M == A.M && B.C == A.C && B.NC == A.NC) {
+        g->G.p[k] = B;
+        idx[k++] = j;
+      }
+    }
+    g->G.n = k;
+#if defined(PC_EMULATE)
+    pc::emu_rt_group(g->G);
+#else
+    if (const cudaError_t e = rt_launch(g->G, A.M, A.C, A.NC, g->st)) {
+      cudaGetLastError();
+      rc = group_fail(g, B200CONV_ECUDA, std::string("group launch: ") + cudaGetErrorString(e));
+      break;
+    }
+#endif
+    g->launches++;
+    for (int j = 0; j < k; ++j) g->launched[idx[j]] = 1;
+  }
+  // commit: head bookkeeping and the tail blocks the calls complete, behind the group's event
+  bool recorded = false;
+  if (waited) {
+    if (cudaEventRecord(g->ev, g->st) != cudaSuccess) {
+      cudaGetLastError();
+      if (!rc) rc = group_fail(g, B200CONV_ECUDA, "group: event record failed");
+    } else {
+      recorded = true;
+    }
+  }
+  for (size_t i = 0; i < n; ++i) {
+    if (!g->launched[i]) continue;
+    if (int crc = rt_commit(g->m[i], g->P[i], g->ev, g->st, &recorded))
+      if (!rc) rc = group_member_fail(g, i, crc);
+  }
+  if (recorded)
+    for (size_t i = 0; i < n; ++i)
+      if (g->prepared[i]) g->m[i]->grp_ev = g->ev;
+  // every other member on its own, while the shared launches run
+  for (size_t i = 0; i < n && !rc; ++i)
+    if (!g->nc[i])
+      if (int mrc = b200conv_process(g->m[i], in[i], out[i], len)) rc = group_member_fail(g, i, mrc);
+  // wait for each launched member's completion word; if one does not show up within 20 ms, synchronise the group
+  // stream once (and report its error)
+  const auto t0 = std::chrono::steady_clock::now();
+  bool synced = false;
+  for (size_t i = 0; i < n; ++i) {
+    if (!g->launched[i]) continue;
+    b200conv* h = g->m[i];
+    volatile unsigned int* f = h->hflag;
+    const unsigned int want = g->P[i].done_val;
+    for (unsigned spins = 0; !synced && (int)(*f - want) < 0; ++spins)
+      if ((spins & 0x3ff) == 0x3ff && std::chrono::steady_clock::now() - t0 > std::chrono::milliseconds(20)) {
+        if (const cudaError_t e = cudaStreamSynchronize(g->st)) {
+          cudaGetLastError();
+          return group_fail(g, B200CONV_ECUDA, std::string("group stream: ") + cudaGetErrorString(e));
+        }
+        synced = true;
+      }
+    const int Cout = h->route_on ? h->n_out : h->C;
+    for (int c = 0; c < Cout; ++c) std::memcpy(out[i][c], h->hpin_out + (size_t)c * len, len * sizeof(float));
+  }
+  return rc;
 }
 
 int b200conv_process_device_sliced(b200conv_t* h, const float* in_dev, size_t in_stride, float* out_dev, size_t out_stride,

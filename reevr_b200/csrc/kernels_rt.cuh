@@ -75,6 +75,15 @@ struct RtParams {
   int mode; const float2* Yt;
 };
 
+// The calls of one shape class of a group, one cluster each (k_rt_group), passed by value: about 23 KB, inside the
+// 32 764-byte kernel-parameter limit of CUDA >= 12.1 on sm_90
+constexpr int kRtGroupMax = 32;
+struct RtGroupParams {
+  int n;
+  RtParams p[kRtGroupMax];
+};
+static_assert(sizeof(RtGroupParams) <= 32764, "k_rt_group's parameter table exceeds the kernel-parameter limit");
+
 // shared-memory layout of one CTA (float2 units unless noted); xnew and yfull hold one row per segment, MB apart
 struct RtSmem {
   int tw, bufA, bufB, xnew, yfull;       // float2 offsets
@@ -234,141 +243,24 @@ __device__ __forceinline__ void rt_inv_passes(float2* in, float2* out, const flo
   }
 }
 
-// launched with cluster dimension (C * NC, 1, 1) = the whole grid; block 256; dynamic smem rt_smem_layout(M, C).bytes
+// one real-time call: launched with cluster dimension (C * NC, 1, 1) = the whole grid
 template <int M>
 __global__ void __launch_bounds__(256) k_rt_block(RtParams P) {
-  extern __shared__ __align__(16) unsigned char pc_rt_smem[];
-  const RtSmem L = rt_smem_layout(M, P.C);
-  constexpr int MB = M < 16 ? 16 : M;
-  float2* sm2 = reinterpret_cast<float2*>(pc_rt_smem);
-  float2* tw = sm2 + L.tw;
-  float2* bufA = sm2 + L.bufA;
-  float2* bufB = sm2 + L.bufB;
-  float* xs = reinterpret_cast<float*>(pc_rt_smem + L.xs);
-  float* ys = reinterpret_cast<float*>(pc_rt_smem + L.ys);
-  float4* red = reinterpret_cast<float4*>(pc_rt_smem + L.red);
-  float* mixbuf = reinterpret_cast<float*>(pc_rt_smem + L.mixbuf);
-  const int tid = threadIdx.x;
-  const int rank = blockIdx.x, c = rank / P.NC, q = rank % P.NC;
-  const bool remote_stores = (P.mode == 0) || (P.mode == 2 && P.mix_on);     // uniform over the cluster
-  if (remote_stores) rt_cluster_arrive();
-  for (int j = tid; j < tw_table_len(M); j += 256) tw[j] = P.tw[j];
+  const int rank = blockIdx.x;
+#include "kernels_rt_step.inc"
+}
 
-  for (int g = 0; g < P.nseg; ++g) {
-    const RtSeg& S = P.seg[g];
-    float2* xnew = sm2 + L.xnew + g * MB;
-    float2* yfull = sm2 + L.yfull + g * MB;
-    if (P.mode != 2) {
-      // ---- A: the segment's block.  The q = 0 CTA overwrites the head's open block in the second segment only after
-      // the cluster barrier of the first, so every CTA has read its earlier samples by then.
-      for (int i = tid; i < M; i += 256) rt_assemble(P, S, c, q, i, xs);
-      __syncthreads();
-
-      // ---- B: forward real FFT -> xnew
-      if constexpr (M == 1) {
-        if (tid == 0) { bufA[0] = make_float2(xs[0], 0.0f); }
-        __syncthreads();
-        if (tid == 0) fwd_split(bufA, xnew, tw, M, 0);
-      } else {
-        constexpr int R0 = pass_radix(M, 1);
-        for (int i = tid; i < M / R0; i += 256)
-          stockham_butterfly<false>(RtSmemIn{xs, S.fill + S.len}, SmemOut{bufA}, tw + tw_pass_offset(M, 1), M, 1, R0, i);
-        __syncthreads();
-        float2* res = rt_fwd_passes<M, R0>(bufA, bufB, tw, tid);
-        for (int k = tid; k <= M / 2; k += 256) fwd_split(res, xnew, tw, M, k);
-      }
-      __syncthreads();
-      if (q == 0) {
-        float2* row = P.X + (long long)c * P.x_cstride + S.head * (long long)M;
-        for (int k = tid; k < M; k += 256) row[k] = xnew[k];
-      }
-      if (P.mode == 1) return;          // FRONT: the sweep is a separate all-SM launch (uniform across the cluster)
-    }
-
-    const float2* Yt_src = yfull;
-    if (P.mode == 0) {
-      // ---- C: sweep of this CTA's bin tile (the second segment's partition 1 is the first segment's spectrum)
-      const int pairs = rt_pairs(M, P.NC);
-      const int PG = 256 / pairs;               // host guarantees 1 <= pairs <= 256
-      const int pi = tid % pairs, pg = tid / pairs;
-      const int k = q * (M / P.NC) + 2 * pi;
-      if (pg < PG) {
-        const float4c r = rt_sweep_thread(P, S.head, c, k, pg, PG, xnew, g ? sm2 + L.xnew : nullptr);
-        red[tid] = make_float4(r.a.x, r.a.y, r.b.x, r.b.y);
-      }
-      __syncthreads();
-      // ---- D: reduce the partition groups, tile -> q = 0 CTA of the convolver (DSMEM), overlap row of the next block
-      if (g == 0) rt_cluster_wait();            // every CTA of the cluster has started
-      if (tid < pairs) {
-        float4 v = red[tid];
-        for (int gg = 1; gg < PG; ++gg) {
-          const float4 u = red[tid + gg * pairs];
-          v.x += u.x; v.y += u.y; v.z += u.z; v.w += u.w;
-        }
-        float2* dst = rt_map_rank(yfull, (unsigned)(c * P.NC));
-        dst[k] = make_float2(v.x, v.y);
-        dst[k + 1] = make_float2(v.z, v.w);
-        if (S.complete) {
-          float2* yn = P.Ynext + (long long)c * P.y_cstride + k;
-          yn[0] = make_float2(v.x, v.y);
-          yn[1] = make_float2(v.z, v.w);
-        }
-      }
-      rt_cluster_sync();
-    } else {                                    // BACK: the sweep's row is in global memory
-      Yt_src = P.Yt + (long long)c * P.y_cstride;
-      if (S.complete && q == 0) {
-        float2* yn = P.Ynext + (long long)c * P.y_cstride;
-        for (int k = tid; k < M; k += 256) yn[k] = Yt_src[k];
-      }
-      __syncthreads();                          // twiddles staged
-    }
-
-    // ---- E: overlap-add in the frequency domain, inverse FFT, output
-    if (q == 0) {
-      const float2* Yp = g ? sm2 + L.yfull : P.Yprev + (long long)c * P.y_cstride;
-      for (int kk = tid; kk <= M / 2; kk += 256) inv_pre(Yt_src, Yp, bufA, tw, M, kk, 1, 0);
-      __syncthreads();
-      const float scale = 1.0f / (float)M;
-      if constexpr (M == 1) {
-        if (tid == 0) { ys[0] = bufA[0].x * scale; }
-        __syncthreads();
-      } else {
-        rt_inv_passes<M, 1>(bufA, bufB, tw, tid, ys, scale);
-      }
-      if (P.mode == 2 && P.mix_on) rt_cluster_wait();      // BACK mode: first remote store of this launch (all CTAs have q = 0)
-      if (P.mix_on) {
-        float* mb = rt_map_rank(mixbuf, 0u) + (long long)c * M + S.off;
-        for (int i = tid; i < S.len; i += 256) mb[i] = rt_out_sample(P, S, c, ys, S.fill + i);
-      } else {
-        float* o = P.out + (long long)c * P.out_stride + S.off;
-        for (int i = tid; i < S.len; i += 256) o[i] = rt_out_sample(P, S, c, ys, S.fill + i);
-      }
-    }
-  }
-  if (P.mix_on) {
-    rt_cluster_sync();
-    if (rank == 0) {
-      for (int j = tid; j < P.n_out * P.len; j += 256) {
-        const int o = j / P.len, i = j % P.len;
-        float acc = 0.0f;
-        for (int cc = 0; cc < P.C; ++cc) {
-          const float mm = P.mix[o * P.C + cc];
-          if (mm != 0.0f) acc = fmaf(mm, mixbuf[(long long)cc * M + i], acc);
-        }
-        P.out[(long long)o * P.out_stride + i] = acc;
-      }
-    }
-  }
-  if (P.done_flag) {
-    // every CTA that wrote output makes its stores visible system-wide, the cluster meets, CTA 0 raises the flag
-    __threadfence_system();
-    rt_cluster_sync();
-    if (rank == 0 && tid == 0) {
-      *reinterpret_cast<volatile unsigned int*>(P.done_flag) = P.done_val;
-      __threadfence_system();
-    }
-  }
+// The real-time calls of up to kRtGroupMax handles of one shape class (same M, C, NC) in one launch
+// (b200conv_group_process): grid n * C * NC, cluster (C * NC, 1, 1); cluster i runs G.p[i] and raises its own member's
+// completion word.  The clusters share nothing and never wait for each other, so a grid with more clusters than the
+// GPU keeps resident runs them in waves.  The table stays in the kernel-parameter space (__grid_constant__: read in
+// place, no local copy), which saves the driver operation of copying it to the device.
+template <int M>
+__global__ void __launch_bounds__(256) k_rt_group(const __grid_constant__ RtGroupParams G) {
+  const int cs = G.p[0].C * G.p[0].NC;
+  const RtParams& P = G.p[blockIdx.x / cs];
+  const int rank = blockIdx.x % cs;
+#include "kernels_rt_step.inc"
 }
 #else
 // CPU emulation (tests/emu): the CTAs of the cluster run phase by phase; a DSMEM store is a store into the other
@@ -486,6 +378,11 @@ inline void emu_rt_block(const RtParams& P) {
     delete[] ct[r].xs; delete[] ct[r].ys; delete[] ct[r].mix; delete[] ct[r].red;
   }
   delete[] ct;
+}
+
+// the clusters of a group launch one after the other
+inline void emu_rt_group(const RtGroupParams& G) {
+  for (int i = 0; i < G.n; ++i) emu_rt_block(G.p[i]);
 }
 #endif
 
