@@ -209,7 +209,7 @@ struct b200conv {
   // tensor-core sweep (kernels_tc.cuh): Toeplitz tile images of one stage's H, per-bin time lines, the bin-major
   // complex result of the groups that merge it into Y rows
   bool opt_tc = std::getenv("B200CONV_NO_TC") == nullptr;
-  void* tc_A = nullptr;              // FP16 images, then the per-line scale exponents (kernels_tc.cuh a_image_bytes)
+  void* tc_A = nullptr;              // FP16 images, then the per-line scale exponents (kernels_tc.cuh a_image_bytes_gauss)
   const void* tc_A_for = nullptr;    // H the images were built from (+ its geometry)
   int tc_A_P = 0, tc_A_B = 0, tc_A_C = 0;
   float* tc_Xt = nullptr;
@@ -869,7 +869,7 @@ bool tc_reserve_all(b200conv* h, const pc::CmacParams& P, int C, float2** yc, si
   const size_t lines = (size_t)C * P.B;
   if (!tc_reserve(h, &h->tc_Xt, &h->tc_Xt_bytes, lines * 2 * (size_t)g.Lt * sizeof(float))) return false;
   if (!tc_reserve(h, yc, yc_bytes, lines * (size_t)tc::yc_stride(g) * sizeof(float2))) return false;
-  const size_t a_bytes = tc::a_image_bytes(lines, tc::nchunk_f16(g.Q)) + lines * sizeof(int);
+  const size_t a_bytes = tc::a_image_bytes_gauss(lines, tc::nchunk_f16(g.Q)) + lines * 2 * sizeof(int);
   if (h->tc_A_for != P.H || h->tc_A_P != P.Ppad || h->tc_A_B != P.B || h->tc_A_C != C || h->tc_A_bytes < a_bytes) {
     h->tc_A_for = nullptr;
     if (!tc_reserve(h, &h->tc_A, &h->tc_A_bytes, a_bytes)) return false;
@@ -895,12 +895,12 @@ int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C, const TcDirect* 
   if (*reinterpret_cast<volatile int*>(h->tc_err) != 0)
     return fail(h, B200CONV_ECUDA, "tensor-core sweep: a pipeline barrier timed out (code " + std::to_string(*h->tc_err) + ")");
   const int nchunk = tc::nchunk_f16(g.Q);
-  const size_t img_bytes = tc::a_image_bytes(lines, nchunk);
+  const size_t img_bytes = tc::a_image_bytes_gauss(lines, nchunk);
   const bool a_stale = h->tc_A_for != P.H || h->tc_A_P != P.Ppad || h->tc_A_B != P.B || h->tc_A_C != C;
   __half* A = static_cast<__half*>(h->tc_A);
   int* eh = reinterpret_cast<int*>(static_cast<unsigned char*>(h->tc_A) + img_bytes);
   if (!h->tc_attr_set) {
-    CU_CHECK(h, cudaFuncSetAttribute(tc::k_tc_sweep, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::kSmemBytesF16));
+    CU_CHECK(h, cudaFuncSetAttribute(tc::k_tc_sweep, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::kSmemBytesGauss));
     h->tc_attr_set = true;
   }
   cudaStream_t st = h->s_launch;
@@ -919,9 +919,9 @@ int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C, const TcDirect* 
   const int split_chunks = sp.nchunk_lo + g.rows * 2 - sp.chunk_hi;
   tc::k_tc_split_x<<<dim3((unsigned)split_chunks, P.B / 32, C), dim3(32, 8), 0, st>>>(sp);
   float2* Yc = d ? d->Yc : h->tc_Yt;
-  tc::SweepParams wp{A, eh, h->tc_Xt, Yc, tc::yc_stride(g), (int)lines, g.ntile, nchunk, g.rows, P.B, h->tc_err_dev};
-  const int total = (int)lines * g.ntile;
-  tc::k_tc_sweep<<<std::min(total, h->n_sm), tc::kThreads, tc::kSmemBytesF16, st>>>(wp);
+  tc::SweepParams wp{A, eh, h->tc_Xt, Yc, tc::yc_stride(g), (int)lines, g.ntile, tc::npair(g), nchunk, g.rows, P.B, h->tc_err_dev};
+  const int total = (int)lines * tc::npair(g);
+  tc::k_tc_sweep<<<std::min(total, h->n_sm), tc::kThreads, tc::kSmemBytesGauss, st>>>(wp);
   if (!d) {
     tc::MergeYParams mp{Yc, tc::yc_stride(g), P.B, P.nblocks, P.Y, P.y_cstride, P.y_rstride, P.yrow0};
     tc::k_tc_merge_y<<<dim3((P.nblocks + 31) / 32, P.B / 32, C), dim3(32, 8), 0, st>>>(mp);

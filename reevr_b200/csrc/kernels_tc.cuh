@@ -10,34 +10,36 @@
 //   D[i][n] = sum_j A[i][j] * B[j][n],   A[i][j] = H[i + Q - j],   B[j][n] = x[64 n - Q + j],   0 <= j < K = Q + 64
 //
 // (Q = P - 1 rounded up to 64) — a GEMM with M = 64 outputs per segment, N = segments, K = Q + 64, one per bin
-// and channel.  The complex product becomes real GEMMs by stacking [Hr ; Hi] into M = 128 rows and running the
-// same A against the real and the imaginary time line (two accumulators D, D2):
-//   y.re = D[0:64] - D2[64:128],  y.im = D[64:128] + D2[0:64]        (entry 0 = DC / Nyquist: y = (D[0:64], D2[64:128]))
-// The sweep issues the transposed product D^T[n][i] = sum_j B[j][n] * A[i][j]: the wgmma A operand is the time-line
-// window (M = 64 segments), the wgmma B operand the whole 128 x 64 Toeplitz image (N = 128).  Consumer warpgroup w
-// owns time line w (re, im), i.e. accumulator D (w = 0) or D2 (w = 1), all 128 rows.
+// and channel.  The complex product takes three real GEMMs (Gauss), with the images [Hr ; Hi ; Hr + Hi] stacked into
+// 192 rows and three time lines xr, xi, xr + xi:
+//   D1 = Hr xr,  D2 = Hi xi,  D3 = (Hr + Hi)(xr + xi);   y.re = D1 - D2,  y.im = D3 - (D1 + D2)
+//   (entry 0 = DC / Nyquist: y = (D1, D2))
+// The sweep issues the transposed products D^T[n][i] = sum_j B[j][n] * A[i][j]: the wgmma A operand is a time-line
+// window (M = 64 segments), the wgmma B operand the 64-row slice of the image that goes with it (N = 64).  Work items
+// are pairs of tiles of one line: MMA warpgroup w takes tile 2m + w, and both read the same image stream.
 //
 // FP32 accuracy comes from the 3xFP16 split: a = a_hi + a_lo, b = b_hi + b_lo (each FP16-exact, round to nearest),
 // and a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi accumulated in FP32 (dropped term ~2^-22 relative).  FP16 has tf32's
 // 11-bit significand, and its MMAs issue at twice the tf32 rate; what it lacks is exponent range, which exact
 // power-of-two scales restore: 2^eh per line (channel, bin) for H, chosen once per IR from the bin's P values, and
-// 2^ex per tile and time line (re / im) for x, chosen from the 80 x 64 samples the tile reads.  Each puts the
-// window's largest magnitude into [2^14, 2^15) (scale_exp); the epilogue multiplies by 2^-(ex + eh).  A sample keeps
-// the full ~2^-22 relative precision while it lies within ~2^-17 of its window's peak; below that its lo part is an
-// FP16 subnormal and the error is absolute, at most ~2^-39 of the window's peak (DESIGN.md §5).
+// 2^ex per tile and time line (re / im / re + im) for x, chosen from the 80 x 64 samples the tile reads; Hr + Hi has
+// its own 2^eh'.  Each puts the window's largest magnitude into [2^14, 2^15) (scale_exp); the epilogue multiplies each
+// product by its own 2^-(ex + eh).  A sample keeps the full ~2^-22 relative precision while it lies within ~2^-17 of
+// its window's peak; below that its lo part is an FP16 subnormal and the error is absolute, at most ~2^-39 of the
+// window's peak (DESIGN.md §5).
 //
 // The time-line operand of chunk c (64 values of j) is a ROW-SHIFTED WINDOW of one shared-memory strip.  The bin's
 // time line is stored as rows of 64 samples; B[64c + jj][n] = x[64 (n + c) + jj - Q] is row n + c of the strip, i.e.
 // the same SWIZZLE_128B K-major strip (rows of 64 halves = 128 B) with the descriptor start address advanced by
 // c * 128 bytes: the 128-byte swizzle is a function of the absolute shared-memory address, so a start address inside
 // the 1024-byte swizzle atom reads the rows it names.  One 80-row strip per time line and hi / lo part feeds all K
-// chunks of a 64-segment tile: the producer warpgroup bulk-copies the tile's FP32 rows (one contiguous 20 KB piece per
-// time line), picks ex and writes the FP16 hi / lo strips into one of two buffers while the MMA warpgroups work on the
-// previous tile.  The Toeplitz images of H (16 KB, pre-swizzled, 1-D bulk copies) stream through a 4-stage ring.
+// chunks of a 64-segment tile.  Each MMA warpgroup owns six strips (60 KB); between pairs it reads its next tile's FP32
+// rows from global memory (asked into L2 while the previous pair ran), picks ex and writes the strips itself.  The
+// Toeplitz images of H (24 KB per chunk and hi / lo part, pre-swizzled, 1-D bulk copies) stream through a 3-stage ring.
 //
 // Kernels: k_tc_build_a (H -> FP16 hi/lo Toeplitz tile images and eh, once per IR), k_tc_split_x (timeline rows ->
-// per-bin FP32 time lines), k_tc_sweep (producer warpgroup: image ring + strip conversion / two MMA warpgroups
-// accumulating in registers; the epilogue combines the complex product into bin-major float2 lines), k_tc_merge_y
+// per-bin FP32 time lines), k_tc_sweep (a producer warp streams the image ring / two MMA warpgroups convert their
+// strips and accumulate in registers; the epilogue combines the complex product into bin-major float2 lines), k_tc_merge_y
 // (bin-major lines -> Y rows, for the groups whose inverse FFT reads rows).
 #pragma once
 
@@ -124,8 +126,26 @@ PC_TC_HD size_t xf_index(long long line, int comp, long long tau, int rows) {
 constexpr int kYLead = 8;
 PC_TC_HD long long yc_stride(const Geom& g) { return g.Lty + 2 * kYLead; }
 
-// Toeplitz images: [line][chunk][hi, lo][128 rows x 64 halves], then eh of every line (int)
+// Toeplitz images of the four-product form: [line][chunk][hi, lo][128 rows x 64 halves]
 PC_TC_HD size_t a_image_bytes(size_t lines, int nchunk) { return lines * (size_t)nchunk * 2 * kATileBytes; }
+
+// ---- three-product (Gauss) form: what k_tc_sweep runs ------------------------------------------------------------
+// kATileBytes, kAStages, kStageBytes, kSmemBytesF16, kStripThreads and a_image_bytes above describe the four-product
+// form it replaced; tests/test_tc_f16_layout.py reads them.
+constexpr int kGRows = 192;                         // image rows: [Hr ; Hi ; Hr + Hi], 64 output steps each
+constexpr int kGSliceBytes = 64 * 128;              // one 64-row slice (8 KB, a multiple of the 1024-byte swizzle atom)
+constexpr int kGImageBytes = kGRows * 128;          // 24 KB: one chunk's hi or lo image, one ring stage
+constexpr int kGStages = 3;
+constexpr int kGStripBytes = 6 * kStripBytes;       // per MMA warpgroup: re, im, re + im lines x hi, lo strips (60 KB)
+constexpr int kSmemBytesGauss = 2 * kGStripBytes + kGStages * kGImageBytes + 1024;
+constexpr int kGProducts = 3;
+
+// Toeplitz images: [line][chunk][hi, lo][192 rows x 64 halves], then eh of every line ([line][Hr / Hi, Hr + Hi] int)
+PC_TC_HD size_t a_image_bytes_gauss(size_t lines, int nchunk) { return lines * (size_t)nchunk * 2 * kGImageBytes; }
+// work items: pairs of consecutive 64-segment tiles of one line (the last pair of an odd tile count has one)
+PC_TC_HD int npair(const Geom& g) { return (g.ntile + 1) / 2; }
+// 64-sample rows of the FP32 time lines that pair m reads (tiles 2m and 2m + 1 overlap in 16 rows)
+PC_TC_HD int pair_rows(int ntile, int m) { return (2 * m + 1 < ntile ? kN : 0) + kStripRows; }
 
 // power-of-two exponent that puts a window's largest magnitude into [2^14, 2^15).  m = bit pattern of that magnitude
 // (sign cleared).  Zero and non-finite windows use 0: zeros stay exact zeros, NaN / Inf propagate unscaled.
@@ -150,36 +170,42 @@ struct BuildAParams {
   const float2* H;          // [C][Prows][B]
   long long h_cstride;
   int B, P, Q, nchunk;
-  __half* A;                // [C*B lines][nchunk][hi, lo][128 x 64]: SWIZZLE_128B images of 2^eh H
-  int* eh;                  // [C*B lines]
+  __half* A;                // [C*B lines][nchunk][hi, lo][192 x 64]: SWIZZLE_128B images of 2^eh Hr, 2^eh Hi, 2^eh' (Hr + Hi)
+  int* eh;                  // [C*B lines][eh, eh']
 };
 
-// grid (nchunk, B, C), block 256.  Every chunk's CTA finds the same eh from the bin's P values (a few KB, once per IR).
+// grid (nchunk, B, C), block 256.  Every chunk's CTA finds the same eh / eh' from the bin's P values (a few KB, once
+// per IR).  Hr + Hi is rounded to FP32 before it is scaled and split.
 __global__ void __launch_bounds__(256) k_tc_build_a(BuildAParams p) {
-  __shared__ uint32_t red[8];
+  __shared__ uint32_t red[8][2];
   const int c = blockIdx.x, k = blockIdx.y, ch = blockIdx.z;
   const long long line = (long long)ch * p.B + k;
   const float2* Hk = p.H + (long long)ch * p.h_cstride + k;
-  uint32_t m = 0;
+  uint32_t m = 0, ms = 0;
   for (int pp = threadIdx.x; pp < p.P; pp += 256) {
     const float2 h = Hk[(long long)pp * p.B];
     m = max(m, max(abs_bits(h.x), abs_bits(h.y)));
+    ms = max(ms, abs_bits(__fadd_rn(h.x, h.y)));
   }
   m = __reduce_max_sync(0xffffffffu, m);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  ms = __reduce_max_sync(0xffffffffu, ms);
+  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5][0] = m; red[threadIdx.x >> 5][1] = ms; }
   __syncthreads();
 #pragma unroll
-  for (int w = 0; w < 8; ++w) m = max(m, red[w]);
-  const int eh = scale_exp(m);
-  if (c == 0 && threadIdx.x == 0) p.eh[line] = eh;
-  __half* hi = p.A + (line * p.nchunk + c) * 2 * (kATileBytes / 2);
-  __half* lo = hi + kATileBytes / 2;
-  for (int idx = threadIdx.x; idx < kATileBytes / 2; idx += 256) {
+  for (int w = 0; w < 8; ++w) { m = max(m, red[w][0]); ms = max(ms, red[w][1]); }
+  const int eh = scale_exp(m), ehs = scale_exp(ms);
+  if (c == 0 && threadIdx.x == 0) { p.eh[2 * line] = eh; p.eh[2 * line + 1] = ehs; }
+  __half* hi = p.A + (line * p.nchunk + c) * 2 * (kGImageBytes / 2);
+  __half* lo = hi + kGImageBytes / 2;
+  for (int idx = threadIdx.x; idx < kGImageBytes / 2; idx += 256) {
     const int mr = idx >> 6, jj = idx & 63;
     const int part = mr >> 6, i = mr & 63;
     const int pp = i + p.Q - (kChunkK * c + jj);
     float v = 0.0f;
-    if (pp >= 0 && pp < p.P) { const float2 h = Hk[(long long)pp * p.B]; v = ldexpf(part ? h.y : h.x, eh); }
+    if (pp >= 0 && pp < p.P) {
+      const float2 h = Hk[(long long)pp * p.B];
+      v = part == 0 ? ldexpf(h.x, eh) : part == 1 ? ldexpf(h.y, eh) : ldexpf(__fadd_rn(h.x, h.y), ehs);
+    }
     const __half vh = __float2half_rn(v);
     const uint32_t off = sw128_h((uint32_t)mr, (uint32_t)jj) >> 1;
     hi[off] = vh;
@@ -262,11 +288,11 @@ __global__ void __launch_bounds__(256) k_tc_merge_y(MergeYParams p) {
 // ---- the sweep -------------------------------------------------------------------------------------------------
 struct SweepParams {
   const __half* A;
-  const int* eh;
+  const int* eh;            // [lines][eh, eh']
   const float* Xt;
   float2* Yc;               // [lines][ystride] complex result, bin-major (kYLead)
   long long ystride;
-  int lines, ntile, nchunk, rows, B;
+  int lines, ntile, npair, nchunk, rows, B;
   int* err;                // (mapped host word) set non-zero when a barrier wait gave up — a bug, not a data condition
 };
 
@@ -295,12 +321,9 @@ __device__ __forceinline__ void bulk_load(void* dst, const void* src, unsigned b
 }
 // orders this thread's generic-proxy shared-memory accesses before later async-proxy ones (bulk copies, wgmma)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// named barrier 1 over the kStripThreads strip converters; true when every one of them passes `ok`
-__device__ __forceinline__ bool strip_sync(bool ok) {
-  uint32_t r;
-  asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.u32 p, %1, 0;\n\tbar.red.and.pred q, 1, %2, p;\n\tselp.u32 %0, 1, 0, q;\n\t}"
-               : "=r"(r) : "r"((uint32_t)ok), "n"(kStripThreads) : "memory");
-  return r != 0;
+// asks L2 for `bytes` (a multiple of 16) of global memory at a 16-byte aligned address; no completion to wait for
+__device__ __forceinline__ void prefetch_l2(const void* src, unsigned bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" :: "l"(src), "r"(bytes) : "memory");
 }
 // wgmma shared-memory descriptor of a SWIZZLE_128B K-major operand (rows of 128 bytes, 8-row groups 1024 bytes
 // apart, base offset 0), split in two words: only the low word (start address in 16-byte units | leading-offset
@@ -310,28 +333,24 @@ __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr & 0
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 // keeps the compiler from moving or copying accumulator registers across the wgmma issue / wait points
-__device__ __forceinline__ void fence_operands(float (&d)[64]) {
+__device__ __forceinline__ void fence_operands(float (&d)[32]) {
 #pragma unroll
-  for (int j = 0; j < 64; ++j) asm volatile("" : "+f"(d[j]) :: "memory");
+  for (int j = 0; j < 32; ++j) asm volatile("" : "+f"(d[j]) :: "memory");
 }
 template <int N>
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
-// d[64 x 128] (+)= A[64 x 16] * B[16 x 128], f16 operands (both K-major) from shared memory, FP32 accumulators in 64
+// d[64 x 64] (+)= A[64 x 16] * B[16 x 64], f16 operands (both K-major) from shared memory, FP32 accumulators in 32
 // registers per thread
-__device__ __forceinline__ void mma_f16(float (&d)[64], uint32_t a_lo, uint32_t b_lo, uint32_t accumulate) {
+__device__ __forceinline__ void mma_f16(float (&d)[32], uint32_t a_lo, uint32_t b_lo, uint32_t accumulate) {
   const uint64_t da = ((uint64_t)kDescHi << 32) | a_lo, db = ((uint64_t)kDescHi << 32) | b_lo;
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
-               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
-               "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
-               "%64, %65, p, 1, 1, 0, 0;\n\t}"
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+               "%32, %33, p, 1, 1, 0, 0;\n\t}"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
                  "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
                  "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
-                 "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
-                 "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
-                 "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
-                 "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
                : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
 // two FP32 values -> their FP16 hi parts and the FP16 rounding of the residuals, packed in pairs
@@ -345,266 +364,228 @@ __device__ __forceinline__ void split_pair(float a, float b, uint32_t& hi, uint3
 
 __device__ __forceinline__ void bar_sync_n(uint32_t id, uint32_t count) { asm volatile("bar.sync %0, %1;" :: "r"(id), "r"(count) : "memory"); }
 
-// Epilogue of MMA warpgroup CP (0: D = x_re [Hr ; Hi], 1: D2 = x_im [Hr ; Hi]) for one tile, acc scaled:
-//   y.re = D[i] - D2[64 + i],  y.im = D[64 + i] + D2[i]     (entry 0 = DC / Nyquist: y = (D[i], D2[64 + i]))
-// Warpgroup CP stores the output steps i in [32 CP, 32 CP + 32): fragment registers 4 j + r with j in KEEP = {4 CP ..
-// 4 CP + 3} (rows m = i) and 8 + KEEP (rows m = 64 + i).  It hands its other registers (j in GIVE and 8 + GIVE) to the
-// partner through `xch` (this tile's strip buffer; per warpgroup [32 registers][128 threads] floats over its own hi / lo
-// strips, which it stopped reading at its wg_wait<0>) and takes the partner's registers of its own positions into them.
-// The leader releases the buffer (`strip_empty`) once its warpgroup has read the partner's half.  The FP32 operations are one
-// __fsub_rn / __fadd_rn per component on the same operands as everywhere else this product is combined.
-template <int CP>
-__device__ __forceinline__ void tc_store_complex(float (&acc)[64], float* xch, unsigned long long* strip_empty, bool leader,
-                                                 bool dc, float2* dst, int wq, int lane, int t128) {
-  constexpr int KEEP = 4 * CP, GIVE = 4 - KEEP;
-  constexpr int kHalf = 2 * kStripBytes / 4;          // a warpgroup's own hi / lo strips: the partner may still read the other's
-  float* mine = xch + CP * kHalf;
-  const float* theirs = xch + (1 - CP) * kHalf;
+// One MMA warpgroup's strips of tile nt: FP32 rows of the re and im time lines -> re + im (one FP32 add) -> max |x| per
+// line -> ex -> FP16 hi / lo SWIZZLE_128B strips [re, im, re + im][hi, lo].  Called once the warpgroup's MMAs on its
+// previous strips are complete; the 80 x 64 samples of each line are read from global memory straight into registers
+// (5 units of 8 samples per thread and line; the ring producer asked L2 for them while the previous pair ran).
+__device__ __forceinline__ void tc_convert_strips(const SweepParams& P, int line, int nt, unsigned char* strips, uint32_t (*red)[kGProducts],
+                                                  int wq, int lane, int t128, uint32_t bar, int (&ex)[kGProducts]) {
+  constexpr int kU = kStripRows * 8 / 128;                // 16-byte units of 8 halves per thread and line
+  const float4* xr = reinterpret_cast<const float4*>(P.Xt + xf_index(line, 0, (long long)nt * kN * 64, P.rows));
+  const float4* xi = reinterpret_cast<const float4*>(P.Xt + xf_index(line, 1, (long long)nt * kN * 64, P.rows));
+  float4 v[kU][2][2];
 #pragma unroll
-  for (int q = 0; q < 4; ++q)
+  for (int k = 0; k < kU; ++k) {
+    const int u = t128 + 128 * k;
+    v[k][0][0] = __ldg(xr + 2 * u); v[k][0][1] = __ldg(xr + 2 * u + 1);
+    v[k][1][0] = __ldg(xi + 2 * u); v[k][1][1] = __ldg(xi + 2 * u + 1);
+  }
+  uint32_t mx[kGProducts] = {0u, 0u, 0u};
 #pragma unroll
-    for (int r = 0; r < 4; ++r) {
-      mine[(q * 4 + r) * 128 + t128] = acc[4 * (GIVE + q) + r];
-      mine[((4 + q) * 4 + r) * 128 + t128] = acc[4 * (8 + GIVE + q) + r];
-    }
-  bar_sync_n(2, 256);
-#pragma unroll
-  for (int q = 0; q < 4; ++q)
-#pragma unroll
-    for (int r = 0; r < 4; ++r) {
-      acc[4 * (GIVE + q) + r] = theirs[(q * 4 + r) * 128 + t128];
-      acc[4 * (8 + GIVE + q) + r] = theirs[((4 + q) * 4 + r) * 128 + t128];
-    }
-  bar_sync_n(3 + CP, 128);
-  if (leader) mbar_arrive1(strip_empty);
-  // register 4 j + r of lane l in warp wq: segment 16 wq + l / 4 + 8 (r / 2), row m = 8 j + 2 (l % 4) + (r % 2)
-  const int n0 = 16 * wq + (lane >> 2), i0 = 2 * (lane & 3);
-#pragma unroll
-  for (int q = 0; q < 4; ++q)
+  for (int k = 0; k < kU; ++k)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      float y[4];
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int r = 2 * h + e;
-        const float own_lo = acc[4 * (KEEP + q) + r], own_hi = acc[4 * (8 + KEEP + q) + r];
-        const float oth_lo = acc[4 * (GIVE + q) + r], oth_hi = acc[4 * (8 + GIVE + q) + r];
-        const float d0 = CP ? oth_lo : own_lo, d1 = CP ? oth_hi : own_hi;     // D[i], D[64 + i]
-        const float e0 = CP ? own_lo : oth_lo, e1 = CP ? own_hi : oth_hi;     // D2[i], D2[64 + i]
-        y[2 * e] = dc ? d0 : __fsub_rn(d0, e1);
-        y[2 * e + 1] = dc ? e1 : __fadd_rn(d1, e0);
-      }
-      *reinterpret_cast<float4*>(dst + (size_t)(n0 + 8 * h) * 64 + 8 * (KEEP + q) + i0) = make_float4(y[0], y[1], y[2], y[3]);
+      const float4 a = v[k][0][h], b = v[k][1][h];
+      mx[0] = max(mx[0], max(max(abs_bits(a.x), abs_bits(a.y)), max(abs_bits(a.z), abs_bits(a.w))));
+      mx[1] = max(mx[1], max(max(abs_bits(b.x), abs_bits(b.y)), max(abs_bits(b.z), abs_bits(b.w))));
+      mx[2] = max(mx[2], max(max(abs_bits(__fadd_rn(a.x, b.x)), abs_bits(__fadd_rn(a.y, b.y))),
+                             max(abs_bits(__fadd_rn(a.z, b.z)), abs_bits(__fadd_rn(a.w, b.w)))));
     }
+#pragma unroll
+  for (int p = 0; p < kGProducts; ++p) {
+    mx[p] = __reduce_max_sync(0xffffffffu, mx[p]);
+    if (lane == 0) red[wq][p] = mx[p];
+  }
+  bar_sync_n(bar, 128);
+#pragma unroll
+  for (int p = 0; p < kGProducts; ++p) ex[p] = scale_exp(max(max(red[0][p], red[1][p]), max(red[2][p], red[3][p])));
+#pragma unroll
+  for (int p = 0; p < kGProducts; ++p) {
+    // 2^ex as two factors: each is a normal float for every ex scale_exp returns, and x * s1 * s2 is exact wherever
+    // the FP16 result can hold it
+    const float s1 = pow2f(ex[p] >> 1), s2 = pow2f(ex[p] - (ex[p] >> 1));
+#pragma unroll
+    for (int k = 0; k < kU; ++k) {
+      const int u = t128 + 128 * k, r = u >> 3, q = u & 7;
+      float f[8];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float4 a = v[k][0][h], b = v[k][1][h];
+        const float4 w = p == 0 ? a : p == 1 ? b : make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w));
+        f[4 * h] = w.x * s1 * s2; f[4 * h + 1] = w.y * s1 * s2; f[4 * h + 2] = w.z * s1 * s2; f[4 * h + 3] = w.w * s1 * s2;
+      }
+      uint4 hi, lo;
+      split_pair(f[0], f[1], hi.x, lo.x);
+      split_pair(f[2], f[3], hi.y, lo.y);
+      split_pair(f[4], f[5], hi.z, lo.z);
+      split_pair(f[6], f[7], hi.w, lo.w);
+      const uint32_t off = sw128_h((uint32_t)r, (uint32_t)(8 * q));
+      *reinterpret_cast<uint4*>(strips + (p * 2 + 0) * kStripBytes + off) = hi;
+      *reinterpret_cast<uint4*>(strips + (p * 2 + 1) * kStripBytes + off) = lo;
+    }
+  }
+  fence_async_smem();                                     // the strips are read by wgmma (async proxy)
+  bar_sync_n(bar, 128);                                   // ... and `red` is free again
 }
 
-// grid: any (persistent, tiles walked round-robin); block 384 = MMA warpgroups 0 and 1 (warps 0-7), producer
-// warpgroup 2 (warp 8 lane 0 streams the Toeplitz images, warps 9-11 stage and convert the time-line strips).
-// Each MMA warpgroup accumulates the products of kFlushF16 chunks in its wgmma registers and adds them to FP32
-// registers (round-to-nearest) between groups: the tensor core's accumulate truncates, so short accumulation chains
-// keep the error at the level of the FFMA sweep (tools/tc_accuracy_model.py).
+// grid: any (persistent, tile pairs walked round-robin); block 384 = MMA warpgroups 0 and 1 (warps 0-7), producer
+// warpgroup 2 (warp 8 lane 0 streams the Toeplitz images; warps 9-11 only give their registers to the MMA warps).
+// Gauss's three-multiplication form of the complex product:
+//   D1 = Hr xr,  D2 = Hi xi,  D3 = (Hr + Hi)(xr + xi);   y.re = D1 - D2,  y.im = D3 - (D1 + D2)
+//   (entry 0 = DC / Nyquist: y = (D1, D2))
+// Warpgroup w takes tile 2m + w of pair m; both read the same image stream, so every image row meets two time-line
+// tiles.  Each product p is an m64n64k16 chain: A = the warpgroup's strip of line p (re, im, re + im) shifted by
+// chunk c, B = slice p of the stage's 192-row image.  Each product accumulates kFlushF16 chunks in its wgmma
+// registers and is added to FP32 registers (round-to-nearest) between chains: the tensor core's accumulate truncates,
+// so short chains keep the error at the level of the FFMA sweep (tools/tc_accuracy_model.py).  Every product's MMAs
+// of a stage are one commit group, and a warpgroup keeps two groups in flight: a product's finished chain is folded
+// while the other two products' groups run.  The strips are single-buffered (60 KB per warpgroup): between pairs each
+// warpgroup stores its results and converts its next strips while the tensor core idles for it.
 __global__ void __launch_bounds__(kThreads, 1) k_tc_sweep(SweepParams P) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  unsigned char* strips = base;                           // [buf][comp][hi, lo] x kStripBytes, FP16 SWIZZLE_128B
-  unsigned char* ring = base + 8 * kStripBytes;
-  float* stage = reinterpret_cast<float*>(ring + kAStages * kATileBytes);   // [comp][kStripRows][64] FP32
-  __shared__ unsigned long long bar_strip_full[2], bar_strip_empty[2], bar_stage, bar_a_full[kAStages], bar_a_empty[kAStages];
-  __shared__ int strip_ex[2][2];                          // [buf][comp]
-  __shared__ uint32_t strip_max[kStripThreads / 32][2];
+  unsigned char* strips = base;                           // [warpgroup][line re, im, re + im][hi, lo] x kStripBytes
+  unsigned char* ring = base + 2 * kGStripBytes;          // kGStages x [192 rows x 64 halves]
+  __shared__ unsigned long long bar_a_full[kGStages], bar_a_empty[kGStages];
+  __shared__ uint32_t strip_max[2][4][kGProducts];        // [warpgroup][warp][line]
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
   if (tid == 0) {
-    for (int b = 0; b < 2; ++b) { mbar_init(&bar_strip_full[b], kStripThreads); mbar_init(&bar_strip_empty[b], 2); }
-    mbar_init(&bar_stage, 1);
-    for (int i = 0; i < kAStages; ++i) { mbar_init(&bar_a_full[i], 1); mbar_init(&bar_a_empty[i], 2); }
+    for (int i = 0; i < kGStages; ++i) { mbar_init(&bar_a_full[i], 1); mbar_init(&bar_a_empty[i], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  const int total = P.lines * P.ntile;
+  const int total = P.lines * P.npair;
 
   if (warp >= 8) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(kProducerRegs));
-    if (warp == 8) {
-      if (lane == 0) {                                    // ---- image ring
-        unsigned it_a = 0;
-        bool ok = true;
-        for (int tile = blockIdx.x; tile < total && ok; tile += gridDim.x) {
-          const __half* Aline = P.A + (size_t)(tile / P.ntile) * P.nchunk * 2 * (kATileBytes / 2);
-          for (int s = 0; s < P.nchunk * 2; ++s, ++it_a) {
-            const unsigned st = it_a % kAStages, use = it_a / kAStages;
-            if (use > 0 && !mbar_wait(&bar_a_empty[st], (use - 1) & 1u)) { *reinterpret_cast<volatile int*>(P.err) = 2; ok = false; break; }
-            mbar_expect(&bar_a_full[st], kATileBytes);
-            bulk_load(ring + st * kATileBytes, Aline + (size_t)s * (kATileBytes / 2), kATileBytes, &bar_a_full[st]);
-          }
+    if (warp == 8 && lane == 0) {                         // ---- image ring
+      unsigned it_a = 0;
+      for (int item = blockIdx.x; item < total; item += gridDim.x) {
+        const int line = item / P.npair, m = item - line * P.npair;
+        // the pair's FP32 time-line rows: the MMA warpgroups read them once this pair's first stages are loaded
+        const unsigned xbytes = (unsigned)pair_rows(P.ntile, m) * 256u;
+        prefetch_l2(P.Xt + xf_index(line, 0, (long long)m * 2 * kN * 64, P.rows), xbytes);
+        prefetch_l2(P.Xt + xf_index(line, 1, (long long)m * 2 * kN * 64, P.rows), xbytes);
+        const __half* Aline = P.A + (size_t)line * P.nchunk * 2 * (kGImageBytes / 2);
+        for (int s = 0; s < P.nchunk * 2; ++s, ++it_a) {
+          const unsigned st = it_a % kGStages, use = it_a / kGStages;
+          if (use > 0 && !mbar_wait(&bar_a_empty[st], (use - 1) & 1u)) { *reinterpret_cast<volatile int*>(P.err) = 2; return; }
+          mbar_expect(&bar_a_full[st], kGImageBytes);
+          bulk_load(ring + st * kGImageBytes, Aline + (size_t)s * (kGImageBytes / 2), kGImageBytes, &bar_a_full[st]);
         }
       }
-      return;
-    }
-    // ---- strips: FP32 rows -> max |x| -> ex -> FP16 hi / lo SWIZZLE_128B strips, double-buffered
-    const int sid = tid - 9 * 32;
-    const float4* stage4 = reinterpret_cast<const float4*>(stage);
-    int n = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++n) {
-      const int line = tile / P.ntile, nt = tile - line * P.ntile;
-      const int buf = n & 1;
-      if (sid == 0) {
-        fence_async_smem();                               // the previous tile's reads of the staging rows come first
-        mbar_expect(&bar_stage, kStageBytes);
-        for (int comp = 0; comp < 2; ++comp)
-          bulk_load(stage + comp * kStripRows * 64, P.Xt + xf_index(line, comp, (long long)nt * kN * 64, P.rows), kStageBytes / 2, &bar_stage);
-      }
-      bool ok = mbar_wait(&bar_stage, (unsigned)n & 1u);
-      uint32_t mx[2] = {0u, 0u};
-#pragma unroll
-      for (int comp = 0; comp < 2; ++comp)
-        for (int u = sid; u < kStripRows * 16 && ok; u += kStripThreads) {
-          const float4 v = stage4[comp * kStripRows * 16 + u];
-          mx[comp] = max(mx[comp], max(max(abs_bits(v.x), abs_bits(v.y)), max(abs_bits(v.z), abs_bits(v.w))));
-        }
-#pragma unroll
-      for (int comp = 0; comp < 2; ++comp) {
-        mx[comp] = __reduce_max_sync(0xffffffffu, mx[comp]);
-        if (lane == 0) strip_max[warp - 9][comp] = mx[comp];
-      }
-      if (!strip_sync(ok)) { if (sid == 0) *reinterpret_cast<volatile int*>(P.err) = 4; break; }
-      int ex[2];
-#pragma unroll
-      for (int comp = 0; comp < 2; ++comp) {
-        uint32_t m = strip_max[0][comp];
-#pragma unroll
-        for (int w = 1; w < kStripThreads / 32; ++w) m = max(m, strip_max[w][comp]);
-        ex[comp] = scale_exp(m);
-      }
-      if (n >= 2) ok = mbar_wait(&bar_strip_empty[buf], (unsigned)((n >> 1) - 1) & 1u);   // tile n - 2's MMAs are done
-      if (ok) {
-        unsigned char* dst = strips + buf * 4 * kStripBytes;
-#pragma unroll
-        for (int comp = 0; comp < 2; ++comp) {
-          // 2^ex as two factors: each is a normal float for every ex scale_exp returns, and x * s1 * s2 is exact
-          // wherever the FP16 result can hold it
-          const float s1 = pow2f(ex[comp] >> 1), s2 = pow2f(ex[comp] - (ex[comp] >> 1));
-          for (int u = sid; u < kStripRows * 8; u += kStripThreads) {      // 16-byte units of 8 halves
-            const int r = u >> 3, q = u & 7;
-            const float4 a = stage4[(comp * kStripRows + r) * 16 + 2 * q];
-            const float4 b = stage4[(comp * kStripRows + r) * 16 + 2 * q + 1];
-            uint4 hi, lo;
-            split_pair(a.x * s1 * s2, a.y * s1 * s2, hi.x, lo.x);
-            split_pair(a.z * s1 * s2, a.w * s1 * s2, hi.y, lo.y);
-            split_pair(b.x * s1 * s2, b.y * s1 * s2, hi.z, lo.z);
-            split_pair(b.z * s1 * s2, b.w * s1 * s2, hi.w, lo.w);
-            const uint32_t off = sw128_h((uint32_t)r, (uint32_t)(8 * q));
-            *reinterpret_cast<uint4*>(dst + (comp * 2 + 0) * kStripBytes + off) = hi;
-            *reinterpret_cast<uint4*>(dst + (comp * 2 + 1) * kStripBytes + off) = lo;
-          }
-        }
-        if (sid == 0) { strip_ex[buf][0] = ex[0]; strip_ex[buf][1] = ex[1]; }
-        fence_async_smem();                               // the strips are read by wgmma (async proxy)
-        mbar_arrive1(&bar_strip_full[buf]);
-      }
-      if (!strip_sync(ok)) { if (sid == 0) *reinterpret_cast<volatile int*>(P.err) = 4; break; }   // staging rows free
     }
     return;
   }
 
-  // ---- MMA warpgroup `comp` (time line re / im against all 128 rows of the stacked [Hr ; Hi] Toeplitz tile)
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(kMmaRegs));   // two accumulator sets + the FP32 sums
-  const int comp = warp >> 2, wq = warp & 3;
-  const bool leader = (tid & 127) == 0;
-  const uint32_t strip_lo = desc_lo(smem_addr(strips)), ring_lo = desc_lo(smem_addr(ring));
+  // ---- MMA warpgroup wg: tile 2m + wg of every pair m, all three products
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(kMmaRegs));   // 3 chain accumulators + 3 FP32 sums
+  const int wg = warp >> 2, wq = warp & 3, t128 = tid & 127;
+  const bool leader = t128 == 0;
+  unsigned char* my_strips = strips + wg * kGStripBytes;
+  const uint32_t strip_lo = desc_lo(smem_addr(my_strips)), ring_lo = desc_lo(smem_addr(ring));
   unsigned it_a = 0;
-  int n = 0;
-  int ex = 0;
-  // Accumulation chains alternate between d0 and d1: the chain of group g is folded into acc once the first stage of
-  // group g + 1 has been committed, so the tensor core keeps working on g + 1 while g drains and is added (same chains,
-  // same order of the FP32 adds as draining each chain before the next one starts).
-  float d0[64], d1[64];
+  float d[kGProducts][32], acc[kGProducts][32];
+  for (int item = blockIdx.x; item < total; item += gridDim.x) {
+    const int line = item / P.npair, nt = 2 * (item - line * P.npair) + wg;
+    const bool live = nt < P.ntile;                       // false: warpgroup 1 on the last pair of an odd tile count
+    int ex[kGProducts] = {0, 0, 0};
+    if (live) tc_convert_strips(P, line, nt, my_strips, strip_max[wg], wq, lane, t128, 2 + wg, ex);
 #pragma unroll
-  for (int j = 0; j < 64; ++j) { d0[j] = 0.0f; d1[j] = 0.0f; }
-  float acc[64];
-  int pending = -1;                                       // ring stage whose MMAs may still be in flight
-  // issues chunks [g0, min(g0 + kFlushF16, nchunk)) into d; folds `prev` (the previous chain, if g0 > 0) into acc as
-  // soon as it is complete.  false: a barrier wait gave up
-  auto chain = [&](float (&d)[64], float (&prev)[64], int g0) -> bool {
-    const int gend = min(g0 + kFlushF16, P.nchunk);
-    const int buf = n & 1;
-    const uint32_t xs = strip_lo + (((buf * 2 + comp) * 2) * kStripBytes >> 4);   // hi strip; lo strip kStripBytes on
-    for (int c = g0; c < gend; ++c) {
-      if (c == 0) {
-        if (!mbar_wait(&bar_strip_full[buf], (unsigned)(n >> 1) & 1u)) { if (leader) *reinterpret_cast<volatile int*>(P.err) = 3; return false; }
-        ex = strip_ex[buf][comp];
-      }
+    for (int p = 0; p < kGProducts; ++p)
+#pragma unroll
+      for (int j = 0; j < 32; ++j) { d[p][j] = 0.0f; acc[p][j] = 0.0f; }   // each chain's first MMA overwrites d
+    int pending = -1;                                     // ring stage whose MMAs may still be in flight
+    for (int c = 0; c < P.nchunk; ++c) {
+      const bool chain0 = c % kFlushF16 == 0;             // first chunk of an accumulation chain
 #pragma unroll
       for (int hl = 0; hl < 2; ++hl, ++it_a) {
-        const unsigned stage = it_a % kAStages, use = it_a / kAStages;
-        if (!mbar_wait(&bar_a_full[stage], use & 1u)) { if (leader) *reinterpret_cast<volatile int*>(P.err) = 5; return false; }
-        __syncwarp();                                     // wgmma is .aligned: the warp issues it converged
-        fence_operands(d);
-        wg_fence();
-        const uint32_t img = ring_lo + stage * (kATileBytes >> 4);
+        const unsigned stage = it_a % kGStages, use = it_a / kGStages;
+        if (!mbar_wait(&bar_a_full[stage], use & 1u)) { if (leader) *reinterpret_cast<volatile int*>(P.err) = 5; wg_wait<0>(); return; }
+        if (!live) {                                      // nothing reads the stage: hand it straight back
+          __syncwarp();
+          if (leader) mbar_arrive1(&bar_a_empty[stage]);
+          continue;
+        }
+        const uint32_t img = ring_lo + stage * (kGImageBytes >> 4);
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const uint32_t xhi = xs + c * 8 + kk * 2, xlo = xhi + (kStripBytes >> 4);   // row shift c, k16 step kk
-          if (hl == 0) {
-            mma_f16(d, xhi, img + kk * 2, (c > g0 || kk > 0) ? 1u : 0u);
-            mma_f16(d, xlo, img + kk * 2, 1u);
-          } else {
-            mma_f16(d, xhi, img + kk * 2, 1u);
+        for (int p = 0; p < kGProducts; ++p) {
+          __syncwarp();                                   // wgmma is .aligned: the warp issues it converged
+          fence_operands(d[p]);
+          wg_fence();
+          const uint32_t xhi = strip_lo + ((p * 2 * kStripBytes) >> 4) + c * 8, xlo = xhi + (kStripBytes >> 4);   // row shift c
+          const uint32_t b = img + p * (kGSliceBytes >> 4);
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            if (hl == 0) {
+              mma_f16(d[p], xhi + kk * 2, b + kk * 2, (chain0 && kk == 0) ? 0u : 1u);
+              mma_f16(d[p], xlo + kk * 2, b + kk * 2, 1u);
+            } else {
+              mma_f16(d[p], xhi + kk * 2, b + kk * 2, 1u);
+            }
+          }
+          wg_commit();
+          fence_operands(d[p]);
+          wg_wait<2>();                                   // every group before the last two is done
+          if (p == 1 && pending >= 0) {                   // ... so the previous stage's three groups are
+            if (leader) mbar_arrive1(&bar_a_empty[pending]);
+            pending = -1;
+          }
+          // ... and so is the last group of product q = p + 1: fold its chain if the next MMAs of q start a new one
+          const int q = (p + 1) % kGProducts;
+          if (p < 2 ? chain0 && hl == 0 && c > 0 : hl == 1 && (c + 1) % kFlushF16 == 0 && c + 1 < P.nchunk) {
+            fence_operands(d[q]);
+#pragma unroll
+            for (int j = 0; j < 32; ++j) acc[q][j] += d[q][j];
           }
         }
-        wg_commit();
-        fence_operands(d);
-        wg_wait<1>();                                     // everything before this stage's MMAs is done
-        fence_operands(d);
-        if (leader && pending >= 0) mbar_arrive1(&bar_a_empty[pending]);
         pending = (int)stage;
-        if (c == g0 && hl == 0 && g0 > 0) {               // the previous chain is complete: fold it
-          fence_operands(prev);
-#pragma unroll
-          for (int j = 0; j < 64; ++j) acc[j] += prev[j];
-        }
       }
     }
-    return true;
-  };
-  for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++n) {
-    const int line = tile / P.ntile, nt = tile - line * P.ntile;
-    const int eh = __ldg(P.eh + line);
+    wg_wait<0>();                                         // the last chains are complete: fold them, hand back the stage
+    if (!live) continue;
 #pragma unroll
-    for (int j = 0; j < 64; ++j) acc[j] = 0.0f;
-    for (int g0 = 0; g0 < P.nchunk; g0 += 2 * kFlushF16) {  // one accumulation chain per group of kFlushF16 chunks
-      if (!chain(d0, d1, g0)) { wg_wait<0>(); return; }
-      if (g0 + kFlushF16 >= P.nchunk) break;
-      if (!chain(d1, d0, g0 + kFlushF16)) { wg_wait<0>(); return; }
+    for (int p = 0; p < kGProducts; ++p) {
+      fence_operands(d[p]);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) acc[p][j] += d[p][j];
     }
-    wg_wait<0>();                                         // the last chain is complete: fold it, hand back the strips
-    fence_operands(d0);
-    fence_operands(d1);
     if (leader) mbar_arrive1(&bar_a_empty[pending]);
-    pending = -1;
-    if ((P.nchunk + kFlushF16 - 1) / kFlushF16 & 1) {     // an odd number of chains ends in d0
+    // undo the operand scales, per product: one exact multiply when 2^-(ex + eh) is a normal float, ldexpf beyond that
+    const int eh = __ldg(P.eh + 2 * line), ehs = __ldg(P.eh + 2 * line + 1);
 #pragma unroll
-      for (int j = 0; j < 64; ++j) acc[j] += d0[j];
-    } else {
+    for (int p = 0; p < kGProducts; ++p) {
+      const int e = ex[p] + (p == 2 ? ehs : eh);
+      if (e >= -127 && e <= 126) {
+        const float s = pow2f(-e);
 #pragma unroll
-      for (int j = 0; j < 64; ++j) acc[j] += d1[j];
+        for (int j = 0; j < 32; ++j) acc[p][j] *= s;
+      } else {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) acc[p][j] = ldexpf(acc[p][j], -e);
+      }
     }
-    // undo the operand scales: one exact multiply when 2^-(ex + eh) is a normal float, ldexpf beyond that
-    const int e = ex + eh;
-    if (e >= -127 && e <= 126) {
-      const float s = pow2f(-e);
-#pragma unroll
-      for (int j = 0; j < 64; ++j) acc[j] *= s;
-    } else {
-#pragma unroll
-      for (int j = 0; j < 64; ++j) acc[j] = ldexpf(acc[j], -e);
-    }
-    float* xch = reinterpret_cast<float*>(strips + (n & 1) * 4 * kStripBytes);
+    // register 4 j + r of lane l in warp wq: segment 16 wq + l / 4 + 8 (r / 2), step i = 8 j + 2 (l % 4) + (r % 2)
     float2* dst = P.Yc + (size_t)line * P.ystride + kYLead + (size_t)nt * kN * 64;
     const bool dc = line % P.B == 0;
-    if (comp == 0) tc_store_complex<0>(acc, xch, &bar_strip_empty[n & 1], leader, dc, dst, wq, lane, tid & 127);
-    else tc_store_complex<1>(acc, xch, &bar_strip_empty[n & 1], leader, dc, dst, wq, lane, tid & 127);
+    const int n0 = 16 * wq + (lane >> 2), i0 = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float y[4];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int r = 4 * j + 2 * h + e;
+          const float d1 = acc[0][r], d2 = acc[1][r], d3 = acc[2][r];
+          y[2 * e] = dc ? d1 : __fsub_rn(d1, d2);
+          y[2 * e + 1] = dc ? d2 : __fsub_rn(d3, __fadd_rn(d1, d2));
+        }
+        *reinterpret_cast<float4*>(dst + (size_t)(n0 + 8 * h) * 64 + 8 * j + i0) = make_float4(y[0], y[1], y[2], y[3]);
+      }
   }
+  wg_wait<0>();
 }
 
 #endif  // __CUDACC__

@@ -8,9 +8,11 @@ shape and batch of bench.py's headline.  Reported per library:
   * step time: CUDA events around one process_device call, L2 flushed before each, the libraries alternated round by
     round (`--rounds` rounds of `--steps` steps each), median and min - max;
   * per-kernel device time per step from torch.profiler (a separate pass after the timed one);
-  * k_tc_sweep's executed tensor rate: tiles x (Q/32 + 2) x 24 MMAs of 2*128*64*8 flop over its profiled time, and
-    that rate over the data sheet's dense FP16 rate (989 TFLOP/s, H100 SXM at 700 W).  The FP16 kernel executes
-    (Q/64 + 1) K chunks x 12 m64n128k16 MMAs (3xFP16 split x 4 k-steps) x 2 time lines: the same flop count;
+  * k_tc_sweep's executed tensor rate: tiles x (Q/64 + 1) K chunks x 18 m64n128k16-equivalents (3 products x
+    4 k-steps x the 3xFP16 split, as m64n64k16) over its profiled time, and that rate over the data sheet's dense FP16
+    rate (989 TFLOP/s, H100 SXM at 700 W).  `k_tc_sweep_tflops_four_product` counts the four real products of the
+    earlier form (24 equivalents per chunk and tile, what bench.py's roofline counts): the executed rate of a build of
+    that form, 4/3 of the executed rate of this one;
   * max |y - y_first| / peak against the first library's output of the same step (a build of the earlier tf32 form as
     the first library shows how far the FP16 form moved the outputs).
 The card's name, power limit and SM clocks are read in the same run.  Needs a GPU; there is no CPU path."""
@@ -48,11 +50,11 @@ def card_info() -> dict:
     return info
 
 
-def tc_flop(P: int, nb: int) -> float:
+def tc_flop(P: int, nb: int, products: int = 3) -> float:
     q = (max(P - 1, 0) + 63) // 64 * 64
-    nchunk = q // 32 + 2
+    nchunk = q // 64 + 1
     ntile = -(-(-(-nb // 64)) // 64)
-    return float(C * BLOCK * ntile * nchunk * 24) * 2.0 * 128 * 64 * 8
+    return float(C * BLOCK * ntile * nchunk * 6 * products) * 2.0 * 128 * 64 * 16
 
 
 def main() -> None:
@@ -138,7 +140,7 @@ def main() -> None:
                 per[ev.key] = per.get(ev.key, 0.0) + t / 1e3 / args.profile_steps
         kernels[name] = dict(sorted(per.items(), key=lambda kv: -kv[1]))
 
-    flop = tc_flop(P, T)
+    flop, flop4 = tc_flop(P, T), tc_flop(P, T, products=4)
     res = {"shape": {"C": C, "block": BLOCK, "partitions": P, "blocks_per_step": T}, "card_before": card_before,
            "card_after": card_after, "libs": {}}
     for name, _ in libs:
@@ -148,6 +150,7 @@ def main() -> None:
             "step_ms_median": statistics.median(ts), "step_ms_min": min(ts), "step_ms_max": max(ts), "steps": len(ts),
             "k_tc_sweep_ms": sweep_ms, "k_tc_sweep_tflops": flop / (sweep_ms * 1e-3) / 1e12 if sweep_ms > 0 else None,
             "k_tc_sweep_frac_of_fp16_dense": flop / (sweep_ms * 1e-3) / 1e12 / FP16_DENSE_TFLOPS if sweep_ms > 0 else None,
+            "k_tc_sweep_tflops_four_product": flop4 / (sweep_ms * 1e-3) / 1e12 if sweep_ms > 0 else None,
             "max_err_vs_" + first: parity[name],
             "kernels_ms_per_step": {k: round(v, 4) for k, v in kernels[name].items()},
         }
