@@ -155,8 +155,27 @@ const char*        b200conv_group_last_error(const b200conv_group_t* g);
 /* in[i] / out[i]: what b200conv_process(members[i], in[i], out[i], len) takes */
 int                b200conv_group_process(b200conv_group_t* g, const float* const* const* in,
                                           float* const* const* out, size_t len);
-/* cluster launches of the group's shared calls (members count only the tail blocks they enqueue) */
+/* launches of the group's shared calls, chain calls included (members count only the tail blocks they enqueue) */
 unsigned long long b200conv_group_launch_count(const b200conv_group_t* g);
+/* Send / wet chain calls of the group: b200conv_chain_group_process(g, dry, ysend, yrev, out, len) is exactly
+ * b200conv_chain_process(members[i], dry[i], ysend ? ysend[i] : NULL, yrev ? yrev[i] : NULL, out[i], len) for every i,
+ * in member order; outputs, filter states, predelay rings and convolver stages are what those calls would leave,
+ * within float rounding.  dry[i] / out[i]: the member's L / R buffers.  A member shares the group's launches when
+ * b200conv_chain_process would run its call as one zero-copy piece through one cluster launch: it has a chain, no fixed
+ * latency and no pending hot swap, len <= the staging size and <= Lmax - head block, the "rt" option on, a head stage
+ * that fits one cluster, and the conditions of b200conv_group_process.  The shared members take one send launch per
+ * 32 members, one cluster launch per shape class and one wet launch per 32 members, and the host waits once, on one
+ * completion word of the group.  Every other member runs its own b200conv_chain_process inside the call.
+ * Errors, checked for every member before anything is enqueued (no member advances): B200CONV_ESTATE for a member
+ * without a chain or without an impulse response, B200CONV_EINVAL for a NULL dry / out table or entry with len > 0,
+ * B200CONV_ECUDA for a member whose CUDA context failed.  len == 0 does nothing. */
+int                b200conv_chain_group_process(b200conv_group_t* g, const float* const* const* dry,
+                                                const float* const* ysend, const float* const* yrev,
+                                                float* const* const* out, size_t len);
+/* Replace member `index` by h, e.g. by the incoming handle of a completed b200conv_chain_swap (state 3), which then
+ * owns the chain.  B200CONV_EINVAL for an index out of range, h NULL, h already a member at another index or on
+ * another device.  Allocates nothing; the outgoing handle stays usable on its own. */
+int                b200conv_group_set_member(b200conv_group_t* g, int index, b200conv_t* h);
 
 /* Introspection --------------------------------------------------------------------------- */
 typedef struct b200conv_stage_info {

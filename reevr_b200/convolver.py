@@ -430,6 +430,41 @@ class Group:
                                                        C.cast(outs, C.POINTER(C.c_void_p)), n))
         return ys
 
+    def chain_process(self, drys, ysends=None, yrevs=None) -> list:
+        """drys[i] = (dryL, dryR) of engines[i] (equally long calls), ysends / yrevs: per-engine envelopes (an entry or
+        the whole list None: 1); returns [(outL, outR), ...] = engines[i].chain_process(...) for every i, with the
+        calls that fit one cluster launch sharing the send, convolver and wet launches (b200conv_chain_group_process)."""
+        m = len(self.engines)
+        if len(drys) != m or any(len(d) != 2 for d in drys):
+            raise ValueError("need (dryL, dryR) per engine")
+        xs = [[np.ascontiguousarray(a, dtype=np.float32) for a in d] for d in drys]
+        n = xs[0][0].size
+        envs = []
+        for es in (ysends, yrevs):
+            if es is not None and len(es) != m:
+                raise ValueError("need one envelope (or None) per engine")
+            envs.append(None if es is None else [None if e is None else np.ascontiguousarray(e, dtype=np.float32)
+                                                  for e in es])
+        if any(a.size != n for x in xs for a in x) or any(e is not None and e.size != n for es in envs if es for e in es):
+            raise ValueError("every buffer of a group call has the same length")
+        ys = [[np.empty(max(n, 1), np.float32)[:n] for _ in range(2)] for _ in range(m)]
+        keep = [[_ptr_array(x), _ptr_array(y)] for x, y in zip(xs, ys)]
+        drs = (C.c_void_p * m)(*[C.cast(k[0], C.c_void_p) for k in keep])
+        outs = (C.c_void_p * m)(*[C.cast(k[1], C.c_void_p) for k in keep])
+        tabs = [None if es is None else (C.c_void_p * m)(*[None if e is None else e.ctypes.data for e in es])
+                for es in envs]
+        if n:
+            self._check(self._l.b200conv_chain_group_process(
+                self._g, C.cast(drs, C.POINTER(C.c_void_p)),
+                *[None if t is None else C.cast(t, C.POINTER(C.c_void_p)) for t in tabs],
+                C.cast(outs, C.POINTER(C.c_void_p)), n))
+        return [(y[0], y[1]) for y in ys]
+
+    def set_member(self, i: int, engine: Engine) -> None:
+        """engines[i] = engine (b200conv_group_set_member), e.g. the incoming engine of a completed chain_swap"""
+        self._check(self._l.b200conv_group_set_member(self._g, i, engine._h))
+        self.engines[i] = engine
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise B200ConvError(f"group process failed ({rc}): {self._l.b200conv_group_last_error(self._g).decode()}")

@@ -2798,6 +2798,16 @@ struct b200conv_group {
   std::vector<int> nc;                   // cluster width of a qualifying member, 0: it runs its own b200conv_process
   std::vector<char> prepared, launched;
   pc::RtGroupParams G;
+  // b200conv_chain_group_process: the shared members' send / wet parameters, the tables of one launch, the group's
+  // pinned completion word (+ its device-side address) and the wet launch's ticket word on the device
+  std::vector<pc::ChainSendParams> sp;
+  std::vector<pc::ChainWetParams> wp;
+  pc::ChainSendGroupParams SG;
+  pc::ChainWetGroupParams WG;
+  unsigned int* flag = nullptr;
+  unsigned int* flag_dev = nullptr;
+  unsigned int epoch = 0;
+  unsigned int* ticket = nullptr;
 };
 
 static int group_fail(b200conv_group* g, int code, const std::string& msg) { g->err = msg; return code; }
@@ -2825,7 +2835,7 @@ b200conv_group_t* b200conv_group_create(b200conv_t* const* members, int n) {
   if (!g) return nullptr;
   try {
     g->m.assign(members, members + n);
-    g->P.resize(n); g->nc.resize(n); g->prepared.resize(n); g->launched.resize(n);
+    g->P.resize(n); g->nc.resize(n); g->prepared.resize(n); g->launched.resize(n); g->sp.resize(n); g->wp.resize(n);
   } catch (...) {
     delete g;
     return nullptr;
@@ -2835,6 +2845,15 @@ b200conv_group_t* b200conv_group_create(b200conv_t* const* members, int n) {
   bool ok = cudaSetDevice(g->device) == cudaSuccess && cudaDeviceGetStreamPriorityRange(&lo, &hi) == cudaSuccess;
   ok = ok && cudaStreamCreateWithPriority(&g->st, cudaStreamNonBlocking, hi) == cudaSuccess;
   ok = ok && cudaEventCreateWithFlags(&g->ev, cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && cudaMallocHost((void**)&g->flag, 64) == cudaSuccess;
+  if (ok) *g->flag = 0;
+#if defined(PC_EMULATE)
+  g->flag_dev = g->flag;
+#else
+  ok = ok && cudaHostGetDevicePointer((void**)&g->flag_dev, g->flag, 0) == cudaSuccess;
+#endif
+  ok = ok && cudaMalloc(&g->ticket, sizeof(unsigned int)) == cudaSuccess;
+  ok = ok && cudaMemsetAsync(g->ticket, 0, sizeof(unsigned int), g->st) == cudaSuccess;
   if (!ok) {
     cudaGetLastError();
     b200conv_group_destroy(g);
@@ -2851,12 +2870,68 @@ void b200conv_group_destroy(b200conv_group_t* g) {
     if (h->grp_ev == g->ev) h->grp_ev = nullptr;        // everything the event covers has completed
   if (g->ev) cudaEventDestroy(g->ev);
   if (g->st) cudaStreamDestroy(g->st);
+  if (g->flag) cudaFreeHost(g->flag);
+  if (g->ticket) cudaFree(g->ticket);
   delete g;
 }
 
 const char* b200conv_group_last_error(const b200conv_group_t* g) { return g ? g->err.c_str() : "null group"; }
 
 unsigned long long b200conv_group_launch_count(const b200conv_group_t* g) { return g ? g->launches : 0; }
+
+// The prepared members' clusters: one k_rt_group launch per shape class (M, C, NC) and kRtGroupMax members, in
+// member order within a class, on the group stream
+static int group_launch_classes(b200conv_group* g) {
+  const size_t n = g->m.size();
+  for (size_t i = 0; i < n; ++i) {
+    if (!g->prepared[i] || g->launched[i]) continue;
+    const pc::RtParams& A = g->P[i];
+    size_t idx[pc::kRtGroupMax];
+    int k = 0;
+    for (size_t j = i; j < n && k < pc::kRtGroupMax; ++j) {
+      const pc::RtParams& B = g->P[j];
+      if (g->prepared[j] && !g->launched[j] && B.M == A.M && B.C == A.C && B.NC == A.NC) {
+        g->G.p[k] = B;
+        idx[k++] = j;
+      }
+    }
+    g->G.n = k;
+#if defined(PC_EMULATE)
+    pc::emu_rt_group(g->G);
+#else
+    if (const cudaError_t e = rt_launch(g->G, A.M, A.C, A.NC, g->st)) {
+      cudaGetLastError();
+      return group_fail(g, B200CONV_ECUDA, std::string("group launch: ") + cudaGetErrorString(e));
+    }
+#endif
+    g->launches++;
+    for (int j = 0; j < k; ++j) g->launched[idx[j]] = 1;
+  }
+  return 0;
+}
+
+// Commit: head bookkeeping and the tail blocks the launched calls complete, behind the group's event (recorded now if
+// the prepare queued a wait); every prepared member keeps the event for its next own call.  *rc keeps the first error.
+static void group_commit(b200conv_group* g, bool waited, int* rc) {
+  const size_t n = g->m.size();
+  bool recorded = false;
+  if (waited) {
+    if (cudaEventRecord(g->ev, g->st) != cudaSuccess) {
+      cudaGetLastError();
+      if (!*rc) *rc = group_fail(g, B200CONV_ECUDA, "group: event record failed");
+    } else {
+      recorded = true;
+    }
+  }
+  for (size_t i = 0; i < n; ++i) {
+    if (!g->launched[i]) continue;
+    if (int crc = rt_commit(g->m[i], g->P[i], g->ev, g->st, &recorded))
+      if (!*rc) *rc = group_member_fail(g, i, crc);
+  }
+  if (recorded)
+    for (size_t i = 0; i < n; ++i)
+      if (g->prepared[i]) g->m[i]->grp_ev = g->ev;
+}
 
 int b200conv_group_process(b200conv_group_t* g, const float* const* const* in, float* const* const* out, size_t len) {
   if (!g) return B200CONV_EINVAL;
@@ -2904,50 +2979,8 @@ int b200conv_group_process(b200conv_group_t* g, const float* const* const* in, f
     g->P[i].done_flag = h->hflag_dev;
     g->P[i].done_val = ++h->flag_epoch;
   }
-  // launch: one per shape class (M, C, NC) and kRtGroupMax members, in member order within a class
-  for (size_t i = 0; i < n && !rc; ++i) {
-    if (!g->prepared[i] || g->launched[i]) continue;
-    const pc::RtParams& A = g->P[i];
-    size_t idx[pc::kRtGroupMax];
-    int k = 0;
-    for (size_t j = i; j < n && k < pc::kRtGroupMax; ++j) {
-      const pc::RtParams& B = g->P[j];
-      if (g->prepared[j] && !g->launched[j] && B.M == A.M && B.C == A.C && B.NC == A.NC) {
-        g->G.p[k] = B;
-        idx[k++] = j;
-      }
-    }
-    g->G.n = k;
-#if defined(PC_EMULATE)
-    pc::emu_rt_group(g->G);
-#else
-    if (const cudaError_t e = rt_launch(g->G, A.M, A.C, A.NC, g->st)) {
-      cudaGetLastError();
-      rc = group_fail(g, B200CONV_ECUDA, std::string("group launch: ") + cudaGetErrorString(e));
-      break;
-    }
-#endif
-    g->launches++;
-    for (int j = 0; j < k; ++j) g->launched[idx[j]] = 1;
-  }
-  // commit: head bookkeeping and the tail blocks the calls complete, behind the group's event
-  bool recorded = false;
-  if (waited) {
-    if (cudaEventRecord(g->ev, g->st) != cudaSuccess) {
-      cudaGetLastError();
-      if (!rc) rc = group_fail(g, B200CONV_ECUDA, "group: event record failed");
-    } else {
-      recorded = true;
-    }
-  }
-  for (size_t i = 0; i < n; ++i) {
-    if (!g->launched[i]) continue;
-    if (int crc = rt_commit(g->m[i], g->P[i], g->ev, g->st, &recorded))
-      if (!rc) rc = group_member_fail(g, i, crc);
-  }
-  if (recorded)
-    for (size_t i = 0; i < n; ++i)
-      if (g->prepared[i]) g->m[i]->grp_ev = g->ev;
+  if (!rc) rc = group_launch_classes(g);
+  group_commit(g, waited, &rc);
   // every other member on its own, while the shared launches run
   for (size_t i = 0; i < n && !rc; ++i)
     if (!g->nc[i])
@@ -3515,26 +3548,44 @@ void chain_move(b200conv* h, b200conv* g) {
 // done_flag (fixed-latency steps): the wet kernel raises it to done_val after its last store (ticket: its last-CTA
 // counter).  *wide_powers != nullptr: the send runs the whole-GPU form (k_chain_wide_*), which builds its matrix powers
 // when *wide_powers is set and clears it.
+// The send and wet parameters of the next piece of n samples of h's chain, and the chain's bookkeeping moved past it:
+// the slope-switch flags (c_six) and the ring position.  b200conv_chain_group_process builds its members' launches
+// here too, so that a group call and a single call cannot drift apart.
+void chain_piece_params(b200conv* h, const float* d_dry, const float* d_send, const float* d_rev, float* d_out,
+                        size_t dry_stride, size_t out_stride, size_t n, pc::ChainSendParams* sp, pc::ChainWetParams* wp) {
+  const size_t L = h->Lmax;
+  *sp = pc::ChainSendParams{};
+  sp->dry = d_dry; sp->dry_stride = (long long)dry_stride; sp->ysend = d_send;
+  sp->conv_in = h->c_conv_in; sp->conv_stride = (long long)L;
+  sp->filt = h->c_filt; sp->filt_stride = (long long)L;
+  sp->state = h->c_state;
+  sp->ring = h->c_ring; sp->ring_stride = (long long)h->c_ring_size; sp->ring_mask = (long long)h->c_ring_size - 1;
+  sp->ring_pos = h->c_ring_pos; sp->delay_floor = h->c_delay_floor; sp->predelay = h->chain_cfg.predelay;
+  sp->n = (long long)n;
+  sp->lc = h->chain_lc; sp->hc = h->chain_hc;
+  // a slope that crossed 6 dB <-> 12 / 24 dB since the state was last filtered: the kernel trades slot 0 and the stash
+  if (sp->lc.on || sp->hc.on) {
+    sp->swap_lc = h->c_six[0] != (sp->lc.slope == 0); sp->swap_hc = h->c_six[1] != (sp->hc.slope == 0);
+    h->c_six[0] = sp->lc.slope == 0; h->c_six[1] = sp->hc.slope == 0;
+  }
+  h->c_ring_pos += (long long)n;
+  *wp = pc::ChainWetParams{};
+  wp->dry = d_dry; wp->dry_stride = (long long)dry_stride;
+  wp->conv = h->dch[0]; wp->conv_stride = (long long)L;
+  wp->yrev = d_rev;
+  wp->out = d_out; wp->out_stride = (long long)out_stride; wp->n = (long long)n;
+  wp->quad_ts = (h->C == 4 && h->chain_cfg.true_stereo) ? 1 : 0;
+  wp->width = h->chain_cfg.width; wp->drygain = h->chain_cfg.drygain; wp->wetgain = h->chain_cfg.wetgain;
+}
+
 int chain_piece(b200conv* h, const float* d_dry, const float* d_send, const float* d_rev, float* d_out, size_t dry_stride,
                 size_t out_stride, size_t n, bool completing, unsigned int* done_flag, unsigned int done_val,
                 unsigned int* ticket, bool* wide_powers = nullptr) {
-  const int C = h->C;
   const size_t L = h->Lmax;
   b200conv* g = h->swap_live ? h->swap_peer : nullptr;
-  pc::ChainSendParams sp{};
-  sp.dry = d_dry; sp.dry_stride = (long long)dry_stride; sp.ysend = d_send;
-  sp.conv_in = h->c_conv_in; sp.conv_stride = (long long)L;
-  sp.filt = h->c_filt; sp.filt_stride = (long long)L;
-  sp.state = h->c_state;
-  sp.ring = h->c_ring; sp.ring_stride = (long long)h->c_ring_size; sp.ring_mask = (long long)h->c_ring_size - 1;
-  sp.ring_pos = h->c_ring_pos; sp.delay_floor = h->c_delay_floor; sp.predelay = h->chain_cfg.predelay;
-  sp.n = (long long)n;
-  sp.lc = h->chain_lc; sp.hc = h->chain_hc;
-  // a slope that crossed 6 dB <-> 12 / 24 dB since the state was last filtered: the kernel trades slot 0 and the stash
-  if (sp.lc.on || sp.hc.on) {
-    sp.swap_lc = h->c_six[0] != (sp.lc.slope == 0); sp.swap_hc = h->c_six[1] != (sp.hc.slope == 0);
-    h->c_six[0] = sp.lc.slope == 0; h->c_six[1] = sp.hc.slope == 0;
-  }
+  pc::ChainSendParams sp;
+  pc::ChainWetParams wp;
+  chain_piece_params(h, d_dry, d_send, d_rev, d_out, dry_stride, out_stride, n, &sp, &wp);
   if (wide_powers) {
     if (!g) sp.filt = nullptr;          // only the incoming convolver of a fading swap reads the undelayed send
     if (int rc = launch_chain_wide(h, sp, *wide_powers, h->s_main)) return rc;
@@ -3542,7 +3593,6 @@ int chain_piece(b200conv* h, const float* d_dry, const float* d_send, const floa
   } else if (int rc = launch_chain_send(h, sp, h->s_main)) {
     return rc;
   }
-  h->c_ring_pos += (long long)n;
   if (g) {
     // the incoming handle runs on its own stream behind the send kernel: warm-up (first piece), then this piece's
     // undelayed send (src/PluginProcessor.cpp:1801-1806)
@@ -3557,13 +3607,6 @@ int chain_piece(b200conv* h, const float* d_dry, const float* d_send, const floa
   }
   // the convolvers: LL, RR[, LR, RL] read the chain's L / R, per-convolver outputs stay on the device
   if (int rc = chain_convolve(h, h->c_conv_in, L, n)) return rc;
-  pc::ChainWetParams wp{};
-  wp.dry = d_dry; wp.dry_stride = (long long)dry_stride;
-  wp.conv = h->dch[0]; wp.conv_stride = (long long)L;
-  wp.yrev = d_rev;
-  wp.out = d_out; wp.out_stride = (long long)out_stride; wp.n = (long long)n;
-  wp.quad_ts = (C == 4 && h->chain_cfg.true_stereo) ? 1 : 0;
-  wp.width = h->chain_cfg.width; wp.drygain = h->chain_cfg.drygain; wp.wetgain = h->chain_cfg.wetgain;
   wp.done_flag = done_flag; wp.done_val = done_val; wp.ticket = ticket;
   if (g) {
     CU_CHECK(h, cudaStreamWaitEvent(h->s_main, g->ev_comp[0], 0));
@@ -3726,6 +3769,168 @@ int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* 
     done += n;
   }
   if (g && h->swap_xfade <= 0) chain_move(h, g);        // src/PluginProcessor.cpp:1823-1826
+  return B200CONV_OK;
+}
+
+// The chain calls of a group (b200conv_chain_group_process).  A member shares the group's launches when
+// b200conv_chain_process would run its call as one zero-copy piece through one cluster launch, and it can share a
+// k_rt_group launch: a chain, no fixed latency, no pending hot swap, and group_ctas > 0.  Its width, else 0.
+static int chain_group_ctas(const b200conv* h, size_t len) {
+  if (!h->chain_on || h->lat_D || h->swap_peer || h->stages.empty() || !h->c_hpin_dev || !h->opt_rt ||
+      len > h->Lmax - h->stages[0].B)
+    return 0;
+  return group_ctas(h, len);
+}
+
+int b200conv_chain_group_process(b200conv_group_t* g, const float* const* const* dry, const float* const* ysend,
+                                 const float* const* yrev, float* const* const* out, size_t len) {
+  if (!g) return B200CONV_EINVAL;
+  if (len == 0) return B200CONV_OK;
+  if (!dry || !out) return group_fail(g, B200CONV_EINVAL, "null buffer");
+  const size_t n = g->m.size();
+  // every member's arguments before anything is enqueued: a refused call advances no member
+  for (size_t i = 0; i < n; ++i) {
+    const b200conv* h = g->m[i];
+    if (h->sticky_cuda_error) return group_member_fail(g, i, B200CONV_ECUDA);
+    if (!h->chain_on) return group_fail(g, B200CONV_ESTATE, "member " + std::to_string(i) + " owns no send / wet chain");
+    if (h->stages.empty() || (h->lat_D && !h->c_lat))
+      return group_fail(g, B200CONV_ESTATE, "member " + std::to_string(i) + " has no impulse response or chain rings");
+    if (!dry[i] || !out[i] || !dry[i][0] || !dry[i][1] || !out[i][0] || !out[i][1])
+      return group_fail(g, B200CONV_EINVAL, "null buffer of member " + std::to_string(i));
+  }
+  if (cudaSetDevice(g->device) != cudaSuccess) {
+    cudaGetLastError();
+    return group_fail(g, B200CONV_ECUDA, "cudaSetDevice failed");
+  }
+  int rc = 0;
+  bool waited = false;
+  size_t shared = 0;
+  // prepare: inputs into the chain's pinned staging, the send / wet parameters, the waits the convolver call needs
+  // and its parameters (input: the predelayed send, outputs: the per-convolver rows, as chain_convolve runs it)
+  for (size_t i = 0; i < n; ++i) {
+    b200conv* h = g->m[i];
+    g->prepared[i] = g->launched[i] = 0;
+    g->nc[i] = chain_group_ctas(h, len);
+    if (!g->nc[i] || rc) continue;
+    if (h->main_unsynced) {
+      cudaError_t e = cudaEventRecord(h->ev_rt, h->s_main);
+      if (e == cudaSuccess) e = cudaStreamWaitEvent(g->st, h->ev_rt, 0);
+      if (e != cudaSuccess) {
+        rc = group_member_fail(g, i, cuda_fail(h, e, "group: ordering behind the member's stream"));
+        continue;
+      }
+      h->main_unsynced = false;
+      waited = true;
+    }
+    const size_t cap = h->hpin_cap;
+    std::memcpy(h->c_hpin, dry[i][0], len * sizeof(float));
+    std::memcpy(h->c_hpin + cap, dry[i][1], len * sizeof(float));
+    const float* ys = ysend ? ysend[i] : nullptr;
+    const float* yr = yrev ? yrev[i] : nullptr;
+    if (ys) std::memcpy(h->c_hpin + 2 * cap, ys, len * sizeof(float));
+    if (yr) std::memcpy(h->c_hpin + 3 * cap, yr, len * sizeof(float));
+    float* d = h->c_hpin_dev;
+    chain_piece_params(h, d, ys ? d + 2 * cap : nullptr, yr ? d + 3 * cap : nullptr, d + 4 * cap, cap, cap, len,
+                       &g->sp[i], &g->wp[i]);
+    h->route_in_only = true;
+    h->s_launch = g->st;                   // a timeline compaction goes to the group stream, ahead of the launches
+    const int prc = rt_prepare(h, g->nc[i], h->c_conv_in, h->Lmax, h->dch[0], h->Lmax, len, g->st, g->P[i], &waited);
+    h->s_launch = h->s_main;
+    h->route_in_only = false;
+    g->prepared[i] = 1;                    // waits may have been queued even if it failed
+    if (prc) { rc = group_member_fail(g, i, prc); continue; }
+    ++shared;
+  }
+  // launch: the sends (one per kChainGroupMax members), the convolvers (one per shape class), the wet mixes (one per
+  // kChainGroupMax members, the last of them raises the group's word), all in member order on the group stream
+  const int T = chain_send_threads(len);
+  const unsigned wet_blocks = (unsigned)((len + 255) / 256);
+  for (size_t i = 0, k = 0; i < n && !rc; ++i) {
+    if (g->prepared[i]) g->SG.p[k++] = g->sp[i];
+    if (k == (size_t)pc::kChainGroupMax || (k && i + 1 == n)) {
+      g->SG.n = (int)k;
+#if defined(PC_EMULATE)
+      pc::emu_chain_send_group(g->SG, T);
+#else
+      pc::k_chain_send_group<<<dim3(2, (unsigned)k), T, 0, g->st>>>(g->SG);
+      if (const cudaError_t e = cudaGetLastError())
+        rc = group_fail(g, B200CONV_ECUDA, std::string("group send launch: ") + cudaGetErrorString(e));
+#endif
+      g->launches++;
+      k = 0;
+    }
+  }
+  if (!rc) rc = group_launch_classes(g);
+  const unsigned int want = g->epoch + 1;
+  for (size_t i = 0, k = 0, done = 0; i < n && !rc; ++i) {
+    if (g->prepared[i]) { g->WG.p[k++] = g->wp[i]; ++done; }
+    if (k == (size_t)pc::kChainGroupMax || (k && done == shared)) {
+      g->WG.n = (int)k;
+      const bool last = done == shared;
+      g->WG.done_flag = last ? g->flag_dev : nullptr;
+      g->WG.done_val = want;
+      g->WG.ticket = g->ticket;
+#if defined(PC_EMULATE)
+      pc::emu_chain_wet_group(g->WG);
+#else
+      pc::k_chain_wet_group<<<dim3(wet_blocks, (unsigned)k), 256, 0, g->st>>>(g->WG);
+      if (const cudaError_t e = cudaGetLastError())
+        rc = group_fail(g, B200CONV_ECUDA, std::string("group wet launch: ") + cudaGetErrorString(e));
+#endif
+      g->launches++;
+      k = 0;
+      if (last) { if (!rc) g->epoch = want; break; }
+    }
+  }
+  group_commit(g, waited, &rc);
+  // every other member on its own, while the shared launches run
+  for (size_t i = 0; i < n && !rc; ++i)
+    if (!g->nc[i])
+      if (int mrc = b200conv_chain_process(g->m[i], dry[i], ysend ? ysend[i] : nullptr, yrev ? yrev[i] : nullptr, out[i],
+                                           len))
+        rc = group_member_fail(g, i, mrc);
+  if (!shared || g->epoch != want) return rc;
+  // one completion word for every shared member; if it does not show up within 20 ms, synchronise the group stream
+  // once (and report its error)
+  volatile unsigned int* f = g->flag;
+  const auto t0 = std::chrono::steady_clock::now();
+  for (unsigned spins = 0; (int)(*f - want) < 0; ++spins)
+    if ((spins & 0x3ff) == 0x3ff && std::chrono::steady_clock::now() - t0 > std::chrono::milliseconds(20)) {
+      if (const cudaError_t e = cudaStreamSynchronize(g->st)) {
+        cudaGetLastError();
+        return group_fail(g, B200CONV_ECUDA, std::string("group stream: ") + cudaGetErrorString(e));
+      }
+      break;
+    }
+  for (size_t i = 0; i < n; ++i) {
+    if (!g->launched[i]) continue;
+    const b200conv* h = g->m[i];
+    for (int ch = 0; ch < 2; ++ch) std::memcpy(out[i][ch], h->c_hpin + (4 + ch) * h->hpin_cap, len * sizeof(float));
+  }
+  return rc;
+}
+
+// A completed b200conv_chain_swap moves the chain to the incoming handle: the caller puts it in the outgoing one's
+// place.  The outgoing handle's next own call must still follow the group's event if it holds it.
+int b200conv_group_set_member(b200conv_group_t* g, int index, b200conv_t* h) {
+  if (!g) return B200CONV_EINVAL;
+  if (index < 0 || (size_t)index >= g->m.size()) return group_fail(g, B200CONV_EINVAL, "member index out of range");
+  if (!h) return group_fail(g, B200CONV_EINVAL, "null member");
+  if (h->cfg.device != g->device) return group_fail(g, B200CONV_EINVAL, "the member is on another device");
+  for (size_t j = 0; j < g->m.size(); ++j)
+    if (g->m[j] == h && (int)j != index) return group_fail(g, B200CONV_EINVAL, "the handle is already a member");
+  b200conv* old = g->m[index];
+  if (old != h && old->grp_ev == g->ev) {
+    cudaError_t e = cudaSetDevice(g->device);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(old->s_main, g->ev, 0);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(old->s_post, g->ev, 0);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      return group_fail(g, B200CONV_ECUDA, std::string("set_member: ") + cudaGetErrorString(e));
+    }
+    old->grp_ev = nullptr;
+  }
+  g->m[index] = h;
   return B200CONV_OK;
 }
 

@@ -7,6 +7,8 @@
 //                  (src/PluginProcessor.cpp:1832-1876)
 //   k_chain_wet_xfade  the same during an IR hot swap: outgoing and incoming convolvers crossfaded per sample before
 //                  the mixdown (src/PluginProcessor.cpp:1799-1838)
+//   k_chain_send_group / k_chain_wet_group  the same for the chain calls of a group of handles
+//                  (b200conv_chain_group_process): one launch of each for up to kChainGroupMax members
 // The IR hot swap's warm-up (src/PluginProcessor.cpp:1694-1756) runs k_chain_send in replay mode (replay_w > 0): the
 // input is gathered from the predelay ring, which holds the filtered, undelayed send, with the reference's warmer index
 // map; the filters start from a zero state; nothing is written to the ring.
@@ -217,6 +219,23 @@ PC_HD void chain_wet_xfade_sample(const ChainWetParams& P, long long i) {
   if (P.quad_ts) { wl += P.conv[3 * P.conv_stride + i] * beta; wr += P.conv[2 * P.conv_stride + i] * beta; }
   chain_wet_mix(P, i, wl, wr);
 }
+
+// The chain calls of up to kChainGroupMax handles in one send and one wet launch (b200conv_chain_group_process),
+// passed by value like RtGroupParams (kernels_rt.cuh).  Every member's wet parameters carry no completion word of
+// their own: the wet launch raises the group's.
+constexpr int kChainGroupMax = 32;
+struct ChainSendGroupParams {
+  int n;
+  ChainSendParams p[kChainGroupMax];
+};
+struct ChainWetGroupParams {
+  int n;
+  unsigned int* done_flag; unsigned int done_val;     // pinned word (nullptr: none), raised after every CTA's stores
+  unsigned int* ticket;                               // device word, 0 between launches
+  ChainWetParams p[kChainGroupMax];
+};
+static_assert(sizeof(ChainSendGroupParams) <= 32764, "k_chain_send_group's parameter table exceeds the kernel-parameter limit");
+static_assert(sizeof(ChainWetGroupParams) <= 32764, "k_chain_wet_group's parameter table exceeds the kernel-parameter limit");
 
 // ---- the whole-GPU send form of long device-pointer pieces (b200conv_chain_process_device) -------------------------
 // The math of k_chain_send, spread over as many CTAs as the piece needs, both channels in one grid: chunks of a fixed
@@ -439,51 +458,16 @@ PC_HD void chain_wet_seg_sample(const ChainWetParams& P, const ChainSeg& g, long
 #if defined(__CUDACC__)
 // grid (2 channels), block T threads (T = 64 for real-time calls, 1024 for batches); static smem
 static __global__ void __launch_bounds__(1024) k_chain_send(ChainSendParams P) {
-  __shared__ double AL[kChainStates][kChainStates];    // A^L, column j in AL[.][j]
-  __shared__ float Z[1024][kChainStates];              // pass 1: zero-state end points ; after the scan: initial states
-  const int ch = blockIdx.x, t = threadIdx.x, T = blockDim.x;
-  const long long L = (P.n + T - 1) / T;
-  const long long i0 = (long long)t * L < P.n ? (long long)t * L : P.n;
-  const long long i1 = i0 + L < P.n ? i0 + L : P.n;
-  const bool filtered = P.lc.on || P.hc.on;
-  float* filt = P.filt + (long long)ch * P.filt_stride;
-  if (filtered) {
-    float s[kChainStates];
-#pragma unroll
-    for (int q = 0; q < kChainStates; ++q) s[q] = 0.0f;
-    chain_run_chunk(P, ch, i0, i1, s, nullptr);
-#pragma unroll
-    for (int q = 0; q < kChainStates; ++q) Z[t][q] = s[q];
-    if (t < kChainStates) {
-      double col[kChainStates];
-      chain_power_column(P, L, t, col);
-#pragma unroll
-      for (int q = 0; q < kChainStates; ++q) AL[q][t] = col[q];
-    }
-    __syncthreads();
-    if (t == 0) {       // S_{t+1} = A^L S_t + Z_t ; Z[t] becomes the initial state of chunk t
-      double S[kChainStates];
-      chain_scan_start(P, ch, S);
-      for (int c = 0; c < T; ++c)                      // a ragged / empty last chunk does not advance by A^L
-        chain_scan_step(AL, Z[c], S, (long long)c * L + L <= P.n);
-    }
-    __syncthreads();
-#pragma unroll
-    for (int q = 0; q < kChainStates; ++q) s[q] = Z[t][q];
-    chain_run_chunk(P, ch, i0, i1, s, filt);
-    // the state after the LAST sample of the call belongs to the thread whose chunk ends at n
-    if (i1 == P.n && i0 < P.n) {
-#pragma unroll
-      for (int q = 0; q < kChainStates; ++q) P.state[ch * kChainStateStride + q] = s[q];
-    }
-  } else {
-    for (long long i = i0; i < i1; ++i) filt[i] = chain_send_in(P, ch, i);
-  }
-  if (P.replay_w) return;
-  __syncthreads();
-  for (long long i = t; i < P.n; i += T) chain_ring_write(P, ch, i);
-  __syncthreads();
-  for (long long i = t; i < P.n; i += T) chain_ring_read(P, ch, i);
+  const int ch = blockIdx.x;
+#include "kernels_chain_send.inc"
+}
+
+// The send of up to kChainGroupMax handles' chain calls of one length (b200conv_chain_group_process): grid (2, n),
+// block chain_send_threads(n samples); CTA (ch, i) runs channel ch of G.p[i] exactly as k_chain_send would.
+static __global__ void __launch_bounds__(1024) k_chain_send_group(const __grid_constant__ ChainSendGroupParams G) {
+  const ChainSendParams& P = G.p[blockIdx.y];
+  const int ch = blockIdx.x;
+#include "kernels_chain_send.inc"
 }
 
 // the pattern of k_rt_block's done_flag across the CTAs of a grid: every thread's stores are released system-wide, the
@@ -510,6 +494,24 @@ static __global__ void k_chain_wet_xfade(ChainWetParams P) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < P.n) chain_wet_xfade_sample(P, i);
   chain_wet_done(P);
+}
+
+// The wet mix of up to kChainGroupMax handles' chain calls (b200conv_chain_group_process): grid (blocks of 256
+// samples, n), row i of the grid mixes G.p[i] as k_chain_wet would.  The CTA that draws the last ticket of the whole
+// grid raises the group's one completion word (none if G.done_flag is nullptr).
+static __global__ void __launch_bounds__(256) k_chain_wet_group(const __grid_constant__ ChainWetGroupParams G) {
+  const ChainWetParams& P = G.p[blockIdx.y];
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < P.n) chain_wet_sample(P, i);
+  if (!G.done_flag) return;
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x == 0 && atomicAdd(G.ticket, 1u) == gridDim.x * gridDim.y - 1) {
+    atomicExch(G.ticket, 0u);
+    __threadfence_system();
+    *reinterpret_cast<volatile unsigned int*>(G.done_flag) = G.done_val;
+    __threadfence_system();
+  }
 }
 
 // whole-GPU send form (see above).  One CTA of 64 threads: A, then kWideLogLc + kWidePowers - 1 squarings
@@ -1250,6 +1252,13 @@ inline void emu_chain_wet(const ChainWetParams& P) {
 inline void emu_chain_wet_xfade(const ChainWetParams& P) {
   for (long long i = 0; i < P.n; ++i) chain_wet_xfade_sample(P, i);
   if (P.done_flag) *P.done_flag = P.done_val;
+}
+inline void emu_chain_send_group(const ChainSendGroupParams& G, int T) {
+  for (int i = 0; i < G.n; ++i) emu_chain_send(G.p[i], T);
+}
+inline void emu_chain_wet_group(const ChainWetGroupParams& G) {
+  for (int i = 0; i < G.n; ++i) emu_chain_wet(G.p[i]);
+  if (G.done_flag) *G.done_flag = G.done_val;
 }
 #endif
 
