@@ -44,6 +44,7 @@
 #include "kernels_rt.cuh"
 #include "kernels_chain.cuh"
 #include "kernels_tc.cuh"
+#include "kernels_lfft.cuh"
 
 namespace {
 
@@ -218,6 +219,11 @@ struct b200conv {
   int* tc_err = nullptr;             // mapped pinned word: a barrier wait of k_tc_sweep gave up
   int* tc_err_dev = nullptr;
   bool tc_attr_set = false;
+  // line-FFT sweep (kernels_lfft.cuh): kN-point spectra of every line of one stage's H, cached like tc_A
+  float2* lf_S = nullptr;
+  const void* lf_S_for = nullptr;
+  int lf_S_P = 0, lf_S_B = 0, lf_S_C = 0;
+  size_t lf_S_bytes = 0;
   bool tc_alloc_failed = false;      // the scratch did not fit once: stay on the FFMA sweep
   int last_variant = 0;              // sweep form the last launch_cmac resolved to (b200conv_last_sweep_variant)
   // slot exchange (fused multi-GPU path), stage 0 of a single-stage handle
@@ -389,6 +395,8 @@ void free_all(b200conv* h) {
   cudaFree(h->dch[0]); h->dch[0] = nullptr;
   cudaFree(h->tc_A); cudaFree(h->tc_Xt); cudaFree(h->tc_Yt);
   h->tc_A = h->tc_Xt = nullptr; h->tc_Yt = nullptr; h->tc_A_for = nullptr; h->tc_A_bytes = h->tc_Xt_bytes = h->tc_Yt_bytes = 0;
+  cudaFree(h->lf_S);
+  h->lf_S = nullptr; h->lf_S_for = nullptr; h->lf_S_bytes = 0;
   if (h->tc_err) cudaFreeHost(h->tc_err);
   h->tc_err = h->tc_err_dev = nullptr; h->tc_alloc_failed = false;
   cudaFree(h->c_io); cudaFree(h->c_conv_in); cudaFree(h->c_filt); cudaFree(h->c_state); cudaFree(h->c_ring);
@@ -827,6 +835,9 @@ int launch_cmac_stream_tma(b200conv* h, const pc::CmacParams& P, int C, int stag
 
 // ---- tensor-core sweep (kernels_tc.cuh) -------------------------------------------------------------------------
 constexpr int kTcMinBlocks = 4096;      // below that a 128-segment tile is mostly padding: the FFMA sweep is faster
+// from here on the line-FFT sweep (kernels_lfft.cuh) replaces the tensor-core one; between the two thresholds the
+// Toeplitz form stays (its crossover with the line FFTs is not settled below this length)
+constexpr int kLfftMinBlocks = 16384;
 
 // can this sweep run on the tensor cores?  (geometry only; the scratch is allocated by launch_cmac_tc)
 bool tc_eligible(const b200conv* h, const pc::CmacParams& P, int C) {
@@ -862,19 +873,42 @@ struct TcDirect {
 };
 
 #if !defined(PC_EMULATE)
-// the scratch of a tensor-core sweep: time lines, Toeplitz images and the result lines (*yc); false: not enough memory
-bool tc_reserve_all(b200conv* h, const pc::CmacParams& P, int C, float2** yc, size_t* yc_bytes) {
+// the scratch of a tensor-core (40) or line-FFT (41) sweep: time lines, the result lines (*yc), and the Toeplitz images
+// (40) or line spectra (41); false: not enough memory
+bool tc_reserve_all(b200conv* h, const pc::CmacParams& P, int C, int variant, float2** yc, size_t* yc_bytes) {
   namespace tc = pc::tc;
   const tc::Geom g = tc::make_geom(P.Ppad, P.nblocks);
   const size_t lines = (size_t)C * P.B;
   if (!tc_reserve(h, &h->tc_Xt, &h->tc_Xt_bytes, lines * 2 * (size_t)g.Lt * sizeof(float))) return false;
   if (!tc_reserve(h, yc, yc_bytes, lines * (size_t)tc::yc_stride(g) * sizeof(float2))) return false;
+  if (variant == 41) {
+    const size_t s_bytes = pc::lfft::spectra_bytes(lines, C);
+    if (h->lf_S_for != P.H || h->lf_S_P != P.Ppad || h->lf_S_B != P.B || h->lf_S_C != C || h->lf_S_bytes < s_bytes) {
+      h->lf_S_for = nullptr;
+      if (!tc_reserve(h, &h->lf_S, &h->lf_S_bytes, s_bytes)) return false;
+    }
+    return true;
+  }
   const size_t a_bytes = tc::a_image_bytes_gauss(lines, tc::nchunk_f16(g.Q)) + lines * 2 * sizeof(int);
   if (h->tc_A_for != P.H || h->tc_A_P != P.Ppad || h->tc_A_B != P.B || h->tc_A_C != C || h->tc_A_bytes < a_bytes) {
     h->tc_A_for = nullptr;
     if (!tc_reserve(h, &h->tc_A, &h->tc_A_bytes, a_bytes)) return false;
   }
   return true;
+}
+#endif
+
+#if !defined(PC_EMULATE)
+// the time lines of a tensor-core or line-FFT sweep.  The direct form's forward FFT wrote the group's own blocks
+// (tau = Q + extra ... Q + nblocks - 1) into them: the split only fills the history in front of them and zeroes the
+// tail behind them
+void launch_split_x(b200conv* h, const pc::CmacParams& P, int C, const pc::tc::Geom& g, const TcDirect* d) {
+  namespace tc = pc::tc;
+  tc::SplitXParams sp{P.X, P.x_cstride, P.xrow0 - g.Q, std::max<long long>(0, P.xrow0 - (P.Ppad - 1)), P.xrow0 + P.nblocks, P.B, g.rows, h->tc_Xt,
+                      d ? g.Q + d->extra : g.Lt, d ? g.Q + P.nblocks : g.Lt, 0, 0};
+  tc::split_x_chunks(g.rows, sp.skip_lo, sp.skip_hi, &sp.nchunk_lo, &sp.chunk_hi);
+  const int split_chunks = sp.nchunk_lo + g.rows * 2 - sp.chunk_hi;
+  tc::k_tc_split_x<<<dim3((unsigned)split_chunks, P.B / 32, C), dim3(32, 8), 0, h->s_launch>>>(sp);
 }
 #endif
 
@@ -911,17 +945,44 @@ int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C, const TcDirect* 
     h->tc_A_for = P.H; h->tc_A_P = P.Ppad; h->tc_A_B = P.B; h->tc_A_C = C;
     h->launches++;
   }
-  // the direct form's forward FFT wrote the group's own blocks (tau = Q + extra ... Q + nblocks - 1) into the time
-  // lines: the split only fills the history in front of them and zeroes the tail behind them
-  tc::SplitXParams sp{P.X, P.x_cstride, P.xrow0 - g.Q, std::max<long long>(0, P.xrow0 - (P.Ppad - 1)), P.xrow0 + P.nblocks, P.B, g.rows, h->tc_Xt,
-                      d ? g.Q + d->extra : g.Lt, d ? g.Q + P.nblocks : g.Lt, 0, 0};
-  tc::split_x_chunks(g.rows, sp.skip_lo, sp.skip_hi, &sp.nchunk_lo, &sp.chunk_hi);
-  const int split_chunks = sp.nchunk_lo + g.rows * 2 - sp.chunk_hi;
-  tc::k_tc_split_x<<<dim3((unsigned)split_chunks, P.B / 32, C), dim3(32, 8), 0, st>>>(sp);
+  launch_split_x(h, P, C, g, d);
   float2* Yc = d ? d->Yc : h->tc_Yt;
   tc::SweepParams wp{A, eh, h->tc_Xt, Yc, tc::yc_stride(g), (int)lines, g.ntile, tc::npair(g), nchunk, g.rows, P.B, h->tc_err_dev};
   const int total = (int)lines * tc::npair(g);
   tc::k_tc_sweep<<<std::min(total, h->n_sm), tc::kThreads, tc::kSmemBytesGauss, st>>>(wp);
+  if (!d) {
+    tc::MergeYParams mp{Yc, tc::yc_stride(g), P.B, P.nblocks, P.Y, P.y_cstride, P.y_rstride, P.yrow0};
+    tc::k_tc_merge_y<<<dim3((P.nblocks + 31) / 32, P.B / 32, C), dim3(32, 8), 0, st>>>(mp);
+  }
+  timing_end(h, id);
+  h->launches += d ? 2 : 3;
+  CU_CHECK(h, cudaGetLastError());
+  return 0;
+#endif
+}
+
+// the line-FFT sweep (kernels_lfft.cuh); the scratch is in place (tc_reserve_all); d != nullptr: the B = 512 direct form
+int launch_cmac_lfft(b200conv* h, const pc::CmacParams& P, int C, const TcDirect* d) {
+#if defined(PC_EMULATE)
+  (void)P; (void)C; (void)d;
+  return fail(h, B200CONV_EINVAL, "the line-FFT sweep is not part of the CPU emulation");
+#else
+  namespace tc = pc::tc;
+  namespace lf = pc::lfft;
+  const tc::Geom g = tc::make_geom(P.Ppad, P.nblocks);
+  const lf::Plan plan = lf::make_plan(P.Ppad, P.nblocks);
+  const int lines = C * P.B;
+  cudaStream_t st = h->s_launch;
+  int id = timing_begin(h, kKindCmac);
+  if (h->lf_S_for != P.H || h->lf_S_P != P.Ppad || h->lf_S_B != P.B || h->lf_S_C != C) {   // once per IR (and stage)
+    lf::k_lfft_build_h<<<dim3(P.B, C), lf::kThreads, 0, st>>>(lf::BuildHParams{P.H, P.h_cstride, P.B, P.Ppad, C, h->lf_S});
+    h->lf_S_for = P.H; h->lf_S_P = P.Ppad; h->lf_S_B = P.B; h->lf_S_C = C;
+    h->launches++;
+  }
+  launch_split_x(h, P, C, g, d);
+  float2* Yc = d ? d->Yc : h->tc_Yt;
+  const lf::SweepParams wp{h->tc_Xt, h->lf_S, Yc, tc::yc_stride(g), g.rows, P.B, C, plan};
+  lf::k_lfft_sweep<<<(unsigned)lines * (unsigned)plan.nseg, lf::kThreads, 0, st>>>(wp);
   if (!d) {
     tc::MergeYParams mp{Yc, tc::yc_stride(g), P.B, P.nblocks, P.Y, P.y_cstride, P.y_rstride, P.yrow0};
     tc::k_tc_merge_y<<<dim3((P.nblocks + 31) / 32, P.B / 32, C), dim3(32, 8), 0, st>>>(mp);
@@ -951,14 +1012,15 @@ int select_cmac(b200conv* h, const pc::CmacParams& P, int C, float2** yc, size_t
     }
     else if (P.nblocks <= kStreamNBS && P.B >= 64 && P.Ppad >= 1) variant = 101;
     else if (P.nblocks <= kStreamNBS && P.B >= 2 && P.Ppad >= 1) variant = 100;
-    else if (h->opt_tc && !h->tc_alloc_failed && P.nblocks >= kTcMinBlocks && tc_eligible(h, P, C)) variant = 40;
+    else if (h->opt_tc && !h->tc_alloc_failed && P.nblocks >= kTcMinBlocks && tc_eligible(h, P, C))
+      variant = P.nblocks >= kLfftMinBlocks ? 41 : 40;
     else variant = (P.nblocks >= 64) ? 22 : 26;
   }
-  if (variant == 40) {                         // wgmma 3xFP16 block-Toeplitz sweep
-    if (!tc_eligible(h, P, C)) return fail(h, B200CONV_EINVAL, "tensor-core sweep: unsupported shape (needs B % 32 == 0, at most 961 partitions, no slot exchange)");
+  if (variant == 40 || variant == 41) {        // wgmma 3xFP16 block-Toeplitz sweep / FP32 line FFTs
+    if (!tc_eligible(h, P, C)) return fail(h, B200CONV_EINVAL, "tensor-core / line-FFT sweep: unsupported shape (needs B % 32 == 0, at most 961 partitions, no slot exchange)");
 #if !defined(PC_EMULATE)
-    if (!tc_reserve_all(h, P, C, yc ? yc : &h->tc_Yt, yc ? yc_bytes : &h->tc_Yt_bytes)) {
-      if (h->cfg.cmac_variant == 40) return fail(h, B200CONV_ENOMEM, "tensor-core sweep: scratch allocation failed");
+    if (!tc_reserve_all(h, P, C, variant, yc ? yc : &h->tc_Yt, yc ? yc_bytes : &h->tc_Yt_bytes)) {
+      if (h->cfg.cmac_variant == variant) return fail(h, B200CONV_ENOMEM, "tensor-core / line-FFT sweep: scratch allocation failed");
       variant = (P.nblocks >= 64) ? 22 : 26;   // not enough device memory for the scratch: FFMA sweep
     }
 #else
@@ -973,6 +1035,7 @@ int select_cmac(b200conv* h, const pc::CmacParams& P, int C, float2** yc, size_t
 // runs the sweep form select_cmac chose; td: the B = 512 direct form of a tensor-core launch group
 int launch_cmac_as(b200conv* h, const pc::CmacParams& P, int C, int variant, const TcDirect* td) {
   if (variant == 40) return launch_cmac_tc(h, P, C, td);
+  if (variant == 41) return launch_cmac_lfft(h, P, C, td);
   if (variant == 108) {                        // 6 stages x 2 CTAs/SM, skewed static slices (B200CONV_STREAM_SKEW percent, default 8)
     if (P.nblocks != 1 || P.B < 64) return fail(h, B200CONV_EINVAL, "TMA streaming sweep needs nblocks == 1 and B >= 64");
     static const float skew = [] { const char* e = std::getenv("B200CONV_STREAM_SKEW"); return e ? (float)std::atof(e) / 100.0f : 0.08f; }();
@@ -1854,7 +1917,7 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
       const bool direct_ok = h->cfg.shard_count == 1 && use_fft512(h, B, nb, C, s.tab512);
       int variant = 0;
       if (int rc = select_cmac(h, cp, C, direct_ok ? &s.tcY[yb] : nullptr, &s.tcY_bytes[yb], &variant)) return rc;
-      tc_direct = direct_ok && variant == 40;
+      tc_direct = direct_ok && (variant == 40 || variant == 41);
 
       pc::FwdParams fp = fwd_params(h, s, it.src, it.src_stride, (long long)it.total, nb, it.direct);
       if (tc_direct) {
