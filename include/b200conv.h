@@ -133,8 +133,9 @@ unsigned long long b200conv_latency_waits(const b200conv_t* h);
  * Semantics: b200conv_group_process(g, in, out, len) is exactly b200conv_process(members[i], in[i], out[i], len) for
  * every i, in member order; outputs and handle states are what those calls would leave, within float rounding.
  * A member QUALIFIES for a call when b200conv_process would run it as one cluster launch (a call of at most one head
- * block on a head stage that fits one cluster) and it is unsharded, not in fixed-latency mode, timing is off and it has
- * zero-copy staging and a completion word.  Qualifying members with the same head block, channel count and cluster
+ * block on a head stage that fits one cluster) and it is unsharded, not in fixed-latency mode or in fixed-latency mode
+ * at the group's latency (b200conv_group_set_latency, below), timing is off and it has zero-copy staging and a
+ * completion word.  Qualifying members with the same head block, channel count and cluster
  * width form one shape class: one launch per class (per 32 members), one cluster per member; routing / mixdown, the
  * stages and whether the call crosses a head-block boundary may differ inside a class.  Every other member (split-mode
  * uniform long IRs, C > 8, len above the head block, a latency handle, timing on, a tail shard, no IR, ...) runs its
@@ -163,7 +164,8 @@ unsigned long long b200conv_group_launch_count(const b200conv_group_t* g);
  * in member order; outputs, filter states, predelay rings and convolver stages are what those calls would leave,
  * within float rounding.  dry[i] / out[i]: the member's L / R buffers.  A member shares the group's launches when
  * b200conv_chain_process would run its call as one zero-copy piece through one cluster launch: it has a chain, no fixed
- * latency and no pending hot swap, len <= the staging size and <= Lmax - head block, the "rt" option on, a head stage
+ * latency or fixed latency at the group's latency (then the conditions of b200conv_group_set_latency apply instead of
+ * the length ones) and no pending hot swap, len <= the staging size and <= Lmax - head block, the "rt" option on, a head stage
  * that fits one cluster, and the conditions of b200conv_group_process.  The shared members take one send launch per
  * 32 members, one cluster launch per shape class and one wet launch per 32 members, and the host waits once, on one
  * completion word of the group.  Every other member runs its own b200conv_chain_process inside the call.
@@ -177,6 +179,28 @@ int                b200conv_chain_group_process(b200conv_group_t* g, const float
  * owns the chain.  B200CONV_EINVAL for an index out of range, h NULL, h already a member at another index or on
  * another device.  Allocates nothing; the outgoing handle stays usable on its own. */
 int                b200conv_group_set_member(b200conv_group_t* g, int index, b200conv_t* h);
+/* Fixed latency for the whole group (the host reports one latency for its set of instances).  samples != 0: every
+ * member is checked against b200conv_set_latency's rules first (IR loaded, unsharded, no slot exchange, no pending hot
+ * swap, samples a multiple of its head block and at most 16 of them); a refusal returns B200CONV_ESTATE / B200CONV_EINVAL
+ * with the member's index in b200conv_group_last_error and changes no member.  Then b200conv_set_latency(member,
+ * samples) runs on every member in member order (each is cleared) and the group records `samples`.  If that fails
+ * part-way with a CUDA or memory error, the members before the failing one are switched, the failing one is at zero
+ * latency, the later ones are unchanged, and the group keeps its previous latency.  samples == 0: the members in
+ * fixed-latency mode go back to zero latency (and are cleared), and group calls are those above again.
+ * A member SHARES the steps of a group call when b200conv_latency(member) equals the group's non-zero latency and each
+ * of its head-block steps would be one cluster launch: unsharded, timing off, zero-copy rings, a head stage that fits
+ * one cluster, and for b200conv_chain_group_process chain rings, the "rt" option on and no pending hot swap.  Any call
+ * length works.  Every other member (a latency set later on its own by b200conv_set_latency, init_* or b200conv_reset;
+ * a split-mode uniform long IR; C > 8; ...) runs its own call inside the group call, as above.
+ * Semantics stay those of the group calls: outputs, filter states, rings and b200conv_latency_waits are what the
+ * members' own fixed-latency calls would leave, within float rounding (output D samples late, zeros before).
+ * Steady state of the sharing members: a call whose samples complete no head block of any of them makes no launch, no
+ * event operation and no wait unless an output block is still pending on the device.  A call that completes steps
+ * makes, per round (the r-th step of every member completing more than r head blocks in the call), one k_rt_group
+ * launch per shape class and 32 members, plus for the chain one send launch per send width (one for equal head blocks)
+ * and one wet launch per 32 members, and records one event.  The group call allocates nothing. */
+int                b200conv_group_set_latency(b200conv_group_t* g, size_t samples);
+size_t             b200conv_group_latency(const b200conv_group_t* g);
 
 /* Introspection --------------------------------------------------------------------------- */
 typedef struct b200conv_stage_info {

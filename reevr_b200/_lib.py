@@ -90,6 +90,8 @@ SYMBOLS = [
     ("b200conv_group_launch_count", C.c_ulonglong, [C.c_void_p]),
     ("b200conv_chain_group_process", C.c_int, [C.c_void_p, _PP, _PP, _PP, _PP, C.c_size_t]),
     ("b200conv_group_set_member", C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    ("b200conv_group_set_latency", C.c_int, [C.c_void_p, C.c_size_t]),
+    ("b200conv_group_latency", C.c_size_t, [C.c_void_p]),
     ("b200conv_num_stages", C.c_int, [C.c_void_p]),
     ("b200conv_stage", C.c_int, [C.c_void_p, C.c_int, C.POINTER(StageInfo)]),
     ("b200conv_ir_len", C.c_size_t, [C.c_void_p, C.c_int]),

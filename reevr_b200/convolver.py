@@ -465,6 +465,16 @@ class Group:
         self._check(self._l.b200conv_group_set_member(self._g, i, engine._h))
         self.engines[i] = engine
 
+    def set_latency(self, samples: int) -> None:
+        """One fixed latency for every engine (b200conv_group_set_latency): each engine's set_latency(samples), after
+        all of them were checked; the engines at the group's latency then share their head-block steps in group calls.
+        0: the engines in fixed-latency mode go back to zero latency."""
+        self._check(self._l.b200conv_group_set_latency(self._g, samples))
+
+    @property
+    def latency(self) -> int:
+        return int(self._l.b200conv_group_latency(self._g))
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise B200ConvError(f"group process failed ({rc}): {self._l.b200conv_group_last_error(self._g).decode()}")

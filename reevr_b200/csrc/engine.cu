@@ -2744,53 +2744,71 @@ static int lat_wait(b200conv_t* h, LatRing* r, unsigned int want, bool* waited) 
   return 0;
 }
 
-// One call in fixed-latency mode, in passes of at most r->piece samples: the samples go into the input ring (in[i] ==
-// nullptr: row i reads 1), every head block a pass completes is enqueued by step(k, v) with sequence value v, and the
-// output is read from the output ring D samples behind the input.  Output before sample 0 is zero.
+// A call in fixed-latency mode runs in passes of at most r->piece samples.  Input half of a pass of n samples, samples
+// [done, done + n) of the call: waits until the ring slots the pass writes are free, copies the samples into the input
+// ring (in[i] == nullptr: row i reads 1) and moves r->pos past them.
+static int lat_in(b200conv_t* h, LatRing* r, const float* const* in, int n_in, size_t done, long long n, bool* waited) {
+  const long long B = (long long)r->B, L = (long long)r->len, NS = (long long)r->nslots;
+  const long long p0 = r->pos;
+  // the slots this pass writes are free once the steps that last read them completed
+  for (long long k = p0 / B; k <= (p0 + n - 1) / B; ++k)
+    if (int rc = lat_wait(h, r, r->slot_seq[k % NS], waited)) return rc;
+  for (long long p = p0; p < p0 + n;) {
+    const long long i = p % L, seg = std::min(p0 + n - p, L - i);
+    for (int c = 0; c < n_in; ++c) {
+      float* dst = r->in + (size_t)c * L + i;
+      if (in[c]) std::memcpy(dst, in[c] + done + (p - p0), (size_t)seg * sizeof(float));
+      else std::fill(dst, dst + seg, 1.0f);
+    }
+    p += seg;
+  }
+  r->pos = p0 + n;
+  return 0;
+}
+
+// Output half of the pass whose input began at ring position p0: the output ring read D samples behind the input, into
+// samples [done, done + n) of the call; output before sample 0 is zero.  Every block it reads has been enqueued by
+// the pass's steps, since D >= B; it waits only for one that has not completed.
+static int lat_out(b200conv_t* h, LatRing* r, float* const* out, int n_out, size_t done, long long p0, long long n,
+                   bool* waited) {
+  const long long B = (long long)r->B, D = (long long)h->lat_D, L = (long long)r->len, NS = (long long)r->nslots;
+  const long long q0 = p0 - D, q1 = p0 + n - D;
+  for (long long q = q0; q < q1;) {
+    const size_t o = done + (size_t)(q - q0);
+    if (q < 0) {
+      const long long z = std::min(q1, 0LL) - q;
+      for (int c = 0; c < n_out; ++c) std::memset(out[c] + o, 0, (size_t)z * sizeof(float));
+      q += z;
+      continue;
+    }
+    const long long k = q / B, slot = k % NS, seg = std::min(q1, (k + 1) * B) - q;
+    if (int rc = lat_wait(h, r, r->slot_seq[slot], waited)) return rc;
+    for (int c = 0; c < n_out; ++c)
+      std::memcpy(out[c] + o, r->out + (size_t)c * L + (size_t)(slot * B + (q - k * B)), (size_t)seg * sizeof(float));
+    q += seg;
+  }
+  return 0;
+}
+
+// One call in fixed-latency mode: per pass the input half, one step(k, v) with sequence value v per head block k the
+// pass completes (a group call runs these steps in shared launches instead), and the output half.
 extern "C++" {
 template <class Step>
 static int lat_run(b200conv_t* h, LatRing* r, const float* const* in, int n_in, float* const* out, int n_out, size_t len,
                    Step step) {
-  const long long B = (long long)r->B, D = (long long)h->lat_D, L = (long long)r->len, NS = (long long)r->nslots;
+  const long long B = (long long)r->B, NS = (long long)r->nslots;
   bool waited = false;                                     // a call that waited counts once in latency_waits
   struct Count { b200conv_t* h; const bool& w; ~Count() { if (w) h->lat_waits++; } } count{h, waited};
   for (size_t done = 0; done < len;) {
     const long long n = (long long)std::min(len - done, r->piece);
     const long long p0 = r->pos;
-    // the slots this pass writes are free once the steps that last read them completed
-    for (long long k = p0 / B; k <= (p0 + n - 1) / B; ++k)
-      if (int rc = lat_wait(h, r, r->slot_seq[k % NS], &waited)) return rc;
-    for (long long p = p0; p < p0 + n;) {
-      const long long i = p % L, seg = std::min(p0 + n - p, L - i);
-      for (int c = 0; c < n_in; ++c) {
-        float* dst = r->in + (size_t)c * L + i;
-        if (in[c]) std::memcpy(dst, in[c] + done + (p - p0), (size_t)seg * sizeof(float));
-        else std::fill(dst, dst + seg, 1.0f);
-      }
-      p += seg;
-    }
-    r->pos = p0 + n;
+    if (int rc = lat_in(h, r, in, n_in, done, n, &waited)) return rc;
     for (long long k = p0 / B; k < (p0 + n) / B; ++k) {      // one step per completed head block
       const unsigned int v = ++r->seq;
       if (int rc = step(k, v)) return rc;
       r->slot_seq[k % NS] = v;
     }
-    // output: block k is enqueued by now, since D >= B
-    const long long q0 = p0 - D, q1 = p0 + n - D;
-    for (long long q = q0; q < q1;) {
-      const size_t o = done + (size_t)(q - q0);
-      if (q < 0) {
-        const long long z = std::min(q1, 0LL) - q;
-        for (int c = 0; c < n_out; ++c) std::memset(out[c] + o, 0, (size_t)z * sizeof(float));
-        q += z;
-        continue;
-      }
-      const long long k = q / B, slot = k % NS, seg = std::min(q1, (k + 1) * B) - q;
-      if (int rc = lat_wait(h, r, r->slot_seq[slot], &waited)) return rc;
-      for (int c = 0; c < n_out; ++c)
-        std::memcpy(out[c] + o, r->out + (size_t)c * L + (size_t)(slot * B + (q - k * B)), (size_t)seg * sizeof(float));
-      q += seg;
-    }
+    if (int rc = lat_out(h, r, out, n_out, done, p0, n, &waited)) return rc;
     done += (size_t)n;
   }
   return 0;
@@ -2871,6 +2889,11 @@ struct b200conv_group {
   unsigned int* flag_dev = nullptr;
   unsigned int epoch = 0;
   unsigned int* ticket = nullptr;
+  // fixed-latency group calls (b200conv_group_set_latency): the group's latency (0: none); per member whether it
+  // shares the call's steps, the ring position its current pass began at and whether the call waited for its ring
+  size_t lat_D = 0;
+  std::vector<char> lshare, lwaited;
+  std::vector<long long> lp0;
 };
 
 static int group_fail(b200conv_group* g, int code, const std::string& msg) { g->err = msg; return code; }
@@ -2899,6 +2922,7 @@ b200conv_group_t* b200conv_group_create(b200conv_t* const* members, int n) {
   try {
     g->m.assign(members, members + n);
     g->P.resize(n); g->nc.resize(n); g->prepared.resize(n); g->launched.resize(n); g->sp.resize(n); g->wp.resize(n);
+    g->lshare.resize(n); g->lwaited.resize(n); g->lp0.resize(n);
   } catch (...) {
     delete g;
     return nullptr;
@@ -2929,8 +2953,11 @@ void b200conv_group_destroy(b200conv_group_t* g) {
   if (!g) return;
   cudaSetDevice(g->device);
   if (g->st) cudaStreamSynchronize(g->st);
-  for (b200conv* h : g->m)
+  for (b200conv* h : g->m) {
     if (h->grp_ev == g->ev) h->grp_ev = nullptr;        // everything the event covers has completed
+    for (LatRing* r : {h->lat, h->c_lat})                // ... and every step the group stream held
+      if (r && r->last_st == g->st) r->last_st = h->s_main;
+  }
   if (g->ev) cudaEventDestroy(g->ev);
   if (g->st) cudaStreamDestroy(g->st);
   if (g->flag) cudaFreeHost(g->flag);
@@ -2996,6 +3023,9 @@ static void group_commit(b200conv_group* g, bool waited, int* rc) {
       if (g->prepared[i]) g->m[i]->grp_ev = g->ev;
 }
 
+static int group_lat_passes(b200conv_group* g, const float* const* const* in, const float* const* ysend,
+                            const float* const* yrev, float* const* const* out, size_t len, bool chain);
+
 int b200conv_group_process(b200conv_group_t* g, const float* const* const* in, float* const* const* out, size_t len) {
   if (!g) return B200CONV_EINVAL;
   if (len == 0) return B200CONV_OK;
@@ -3014,7 +3044,8 @@ int b200conv_group_process(b200conv_group_t* g, const float* const* const* in, f
     cudaGetLastError();
     return group_fail(g, B200CONV_ECUDA, "cudaSetDevice failed");
   }
-  int rc = 0;
+  // the members at the group's fixed latency first, in shared steps
+  int rc = group_lat_passes(g, in, nullptr, nullptr, out, len, false);
   bool waited = false;
   // prepare: inputs into the pinned staging, the waits each call needs, its parameters
   for (size_t i = 0; i < n; ++i) {
@@ -3046,7 +3077,7 @@ int b200conv_group_process(b200conv_group_t* g, const float* const* const* in, f
   group_commit(g, waited, &rc);
   // every other member on its own, while the shared launches run
   for (size_t i = 0; i < n && !rc; ++i)
-    if (!g->nc[i])
+    if (!g->nc[i] && !g->lshare[i])
       if (int mrc = b200conv_process(g->m[i], in[i], out[i], len)) rc = group_member_fail(g, i, mrc);
   // wait for each launched member's completion word; if one does not show up within 20 ms, synchronise the group
   // stream once (and report its error)
@@ -3845,6 +3876,189 @@ static int chain_group_ctas(const b200conv* h, size_t len) {
   return group_ctas(h, len);
 }
 
+// The sends of the prepared members: one k_chain_send_group per send width and kChainGroupMax members, in member order
+static int group_chain_sends(b200conv_group* g) {
+  const size_t n = g->m.size();
+  bool sent[64] = {};                    // b200conv_group_create admits at most 64 members
+  for (size_t i = 0; i < n; ++i) {
+    if (!g->prepared[i] || sent[i]) continue;
+    const int T = chain_send_threads((size_t)g->sp[i].n);
+    int k = 0;
+    for (size_t j = i; j < n && k < pc::kChainGroupMax; ++j)
+      if (g->prepared[j] && !sent[j] && chain_send_threads((size_t)g->sp[j].n) == T) {
+        g->SG.p[k++] = g->sp[j];
+        sent[j] = true;
+      }
+    g->SG.n = k;
+#if defined(PC_EMULATE)
+    pc::emu_chain_send_group(g->SG, T);
+#else
+    pc::k_chain_send_group<<<dim3(2, (unsigned)k), T, 0, g->st>>>(g->SG);
+    if (const cudaError_t e = cudaGetLastError())
+      return group_fail(g, B200CONV_ECUDA, std::string("group send launch: ") + cudaGetErrorString(e));
+#endif
+    g->launches++;
+  }
+  return 0;
+}
+
+// The wet mixes of the prepared members: one k_chain_wet_group per kChainGroupMax members, in member order.  The last
+// raises `flag` to `want`; with flag nullptr every row raises its own member's word instead (fixed-latency steps).
+static int group_chain_wets(b200conv_group* g, unsigned int* flag, unsigned int want) {
+  const size_t n = g->m.size();
+  size_t left = 0;
+  for (size_t i = 0; i < n; ++i) left += g->prepared[i] ? 1 : 0;
+  for (size_t i = 0, k = 0; i < n; ++i) {
+    if (g->prepared[i]) { g->WG.p[k++] = g->wp[i]; --left; }
+    if (k == (size_t)pc::kChainGroupMax || (k && !left)) {
+      unsigned blocks = 0;
+      for (size_t j = 0; j < k; ++j) blocks = std::max(blocks, (unsigned)((g->WG.p[j].n + 255) / 256));
+      g->WG.n = (int)k;
+      g->WG.done_flag = left ? nullptr : flag;
+      g->WG.done_val = want;
+      g->WG.ticket = g->ticket;
+#if defined(PC_EMULATE)
+      pc::emu_chain_wet_group(g->WG);
+#else
+      pc::k_chain_wet_group<<<dim3(blocks, (unsigned)k), 256, 0, g->st>>>(g->WG);
+      if (const cudaError_t e = cudaGetLastError())
+        return group_fail(g, B200CONV_ECUDA, std::string("group wet launch: ") + cudaGetErrorString(e));
+#endif
+      g->launches++;
+      k = 0;
+    }
+  }
+  return 0;
+}
+
+// ---- fixed-latency groups (b200conv_group_set_latency) ---------------------------------------------------------------
+// A member shares the steps of a group call when its latency is the group's and each of its steps would be one cluster
+// launch: lat_step's rt_call path, or for the chain chain_convolve's, with chain rings and no pending hot swap.  Its
+// cluster width, else 0.
+static int group_lat_ctas(const b200conv_group* g, const b200conv* h, bool chain) {
+  if (!g->lat_D || h->lat_D != g->lat_D || h->cfg.shard_count != 1 || h->stages.empty()) return 0;
+  if (chain ? (!h->chain_on || !h->c_lat || h->swap_peer || !h->opt_rt) : (!h->lat || !h->hpin_in_dev || !h->hpin_out_dev))
+    return 0;
+  return std::max(rt_cluster_ctas(h, h->stages[0].B), 0);
+}
+
+// The members that share a group call's fixed-latency steps, walked in passes as lat_run walks one call; a pass is at
+// most the smallest ring piece among them.  Per pass: every sharing member's input half; then rounds, round q holding
+// the q-th step of every member that completes more than q head blocks in the pass, each prepared as lat_step (or the
+// step of chain_process_latency) runs it, with the member's ring word and sequence value, then launched together and
+// committed on the group stream, so that each member's steps stay in order; then every sharing member's output half.
+// The group stream is ordered behind a member's own steps by main_unsynced, as in a zero-latency group call; a call
+// that launched steps records the group's event once, and the members keep it for their next own call (set_device).
+// chain: in / ysend / yrev are the chain's dry / ysend / yrev tables.  Sets lshare for the callers.
+static int group_lat_passes(b200conv_group* g, const float* const* const* in, const float* const* ysend,
+                            const float* const* yrev, float* const* const* out, size_t len, bool chain) {
+  const size_t n = g->m.size();
+  size_t piece = 0;
+  for (size_t i = 0; i < n; ++i) {
+    b200conv* h = g->m[i];
+    g->nc[i] = group_lat_ctas(g, h, chain);
+    g->lshare[i] = g->nc[i] > 0;
+    g->lwaited[i] = 0;
+    if (g->lshare[i]) {
+      const LatRing* r = chain ? h->c_lat : h->lat;
+      piece = piece ? std::min(piece, r->piece) : r->piece;
+    }
+  }
+  int rc = 0;
+  bool stepped = false;
+  for (size_t done = 0; done < len && piece && !rc;) {
+    const long long np = (long long)std::min(len - done, piece);
+    long long rounds = 0;
+    for (size_t i = 0; i < n && !rc; ++i) {
+      if (!g->lshare[i]) continue;
+      b200conv* h = g->m[i];
+      LatRing* r = chain ? h->c_lat : h->lat;
+      const float* rows[4] = {};
+      if (chain) { rows[0] = in[i][0]; rows[1] = in[i][1]; rows[2] = ysend ? ysend[i] : nullptr; rows[3] = yrev ? yrev[i] : nullptr; }
+      bool w = false;
+      g->lp0[i] = r->pos;
+      if (int e = lat_in(h, r, chain ? rows : in[i], chain ? 4 : (h->route_on ? h->n_in : h->C), done, np, &w))
+        rc = group_member_fail(g, i, e);
+      if (w) g->lwaited[i] = 1;
+      const long long B = (long long)r->B;
+      rounds = std::max(rounds, (g->lp0[i] + np) / B - g->lp0[i] / B);
+    }
+    for (long long q = 0; q < rounds && !rc; ++q) {
+      bool waited = false;
+      for (size_t i = 0; i < n; ++i) {
+        g->prepared[i] = g->launched[i] = 0;
+        if (!g->lshare[i] || rc) continue;
+        b200conv* h = g->m[i];
+        LatRing* r = chain ? h->c_lat : h->lat;
+        const long long k = g->lp0[i] / (long long)r->B + q;
+        if (k >= (g->lp0[i] + np) / (long long)r->B) continue;
+        if (h->main_unsynced) {
+          cudaError_t e = cudaEventRecord(h->ev_rt, h->s_main);
+          if (e == cudaSuccess) e = cudaStreamWaitEvent(g->st, h->ev_rt, 0);
+          if (e != cudaSuccess) {
+            rc = group_member_fail(g, i, cuda_fail(h, e, "group: ordering behind the member's stream"));
+            continue;
+          }
+          h->main_unsynced = false;
+          waited = true;
+        }
+        const size_t B = r->B, L = r->len, off = (size_t)(k % (long long)r->nslots) * B;
+        const unsigned int v = ++r->seq;
+        int prc;
+        h->s_launch = g->st;               // a timeline compaction goes to the group stream, ahead of the launches
+        if (chain) {
+          const float* d = r->in_dev + off;
+          chain_piece_params(h, d, d + 2 * L, d + 3 * L, r->out_dev + off, L, L, B, &g->sp[i], &g->wp[i]);
+          g->wp[i].done_flag = r->word_dev; g->wp[i].done_val = v; g->wp[i].ticket = r->ticket;
+          h->route_in_only = true;
+          prc = rt_prepare(h, g->nc[i], h->c_conv_in, h->Lmax, h->dch[0], h->Lmax, B, g->st, g->P[i], &waited);
+          h->route_in_only = false;
+        } else {
+          prc = rt_prepare(h, g->nc[i], r->in_dev + off, L, r->out_dev + off, L, B, g->st, g->P[i], &waited);
+          g->P[i].done_flag = r->word_dev; g->P[i].done_val = v;
+        }
+        h->s_launch = h->s_main;
+        g->prepared[i] = 1;                // waits may have been queued even if it failed
+        if (prc) { rc = group_member_fail(g, i, prc); continue; }
+        r->last_st = g->st;                // lat_wait's fallback synchronises the stream that holds the step
+      }
+      if (!rc && chain) rc = group_chain_sends(g);
+      if (!rc) rc = group_launch_classes(g);
+      if (!rc && chain) rc = group_chain_wets(g, nullptr, 0);
+      group_commit(g, waited, &rc);
+      for (size_t i = 0; i < n && !rc; ++i) {
+        if (!g->launched[i]) continue;
+        LatRing* r = chain ? g->m[i]->c_lat : g->m[i]->lat;
+        const long long k = g->lp0[i] / (long long)r->B + q;
+        r->slot_seq[k % (long long)r->nslots] = chain ? g->wp[i].done_val : g->P[i].done_val;
+        stepped = true;
+      }
+    }
+    for (size_t i = 0; i < n && !rc; ++i) {
+      if (!g->lshare[i]) continue;
+      b200conv* h = g->m[i];
+      bool w = false;
+      if (int e = lat_out(h, chain ? h->c_lat : h->lat, out[i], chain ? 2 : (h->route_on ? h->n_out : h->C), done,
+                          g->lp0[i], np, &w))
+        rc = group_member_fail(g, i, e);
+      if (w) g->lwaited[i] = 1;
+    }
+    done += (size_t)np;
+  }
+  if (stepped) {
+    if (cudaEventRecord(g->ev, g->st) != cudaSuccess) {
+      cudaGetLastError();
+      if (!rc) rc = group_fail(g, B200CONV_ECUDA, "group: event record failed");
+    } else {
+      for (size_t i = 0; i < n; ++i)
+        if (g->lshare[i]) g->m[i]->grp_ev = g->ev;
+    }
+  }
+  for (size_t i = 0; i < n; ++i)                 // a call that waited counts once in the member's latency_waits
+    if (g->lwaited[i]) g->m[i]->lat_waits++;
+  return rc;
+}
+
 int b200conv_chain_group_process(b200conv_group_t* g, const float* const* const* dry, const float* const* ysend,
                                  const float* const* yrev, float* const* const* out, size_t len) {
   if (!g) return B200CONV_EINVAL;
@@ -3865,7 +4079,7 @@ int b200conv_chain_group_process(b200conv_group_t* g, const float* const* const*
     cudaGetLastError();
     return group_fail(g, B200CONV_ECUDA, "cudaSetDevice failed");
   }
-  int rc = 0;
+  int rc = group_lat_passes(g, dry, ysend, yrev, out, len, true);
   bool waited = false;
   size_t shared = 0;
   // prepare: inputs into the chain's pinned staging, the send / wet parameters, the waits the convolver call needs
@@ -3906,49 +4120,17 @@ int b200conv_chain_group_process(b200conv_group_t* g, const float* const* const*
   }
   // launch: the sends (one per kChainGroupMax members), the convolvers (one per shape class), the wet mixes (one per
   // kChainGroupMax members, the last of them raises the group's word), all in member order on the group stream
-  const int T = chain_send_threads(len);
-  const unsigned wet_blocks = (unsigned)((len + 255) / 256);
-  for (size_t i = 0, k = 0; i < n && !rc; ++i) {
-    if (g->prepared[i]) g->SG.p[k++] = g->sp[i];
-    if (k == (size_t)pc::kChainGroupMax || (k && i + 1 == n)) {
-      g->SG.n = (int)k;
-#if defined(PC_EMULATE)
-      pc::emu_chain_send_group(g->SG, T);
-#else
-      pc::k_chain_send_group<<<dim3(2, (unsigned)k), T, 0, g->st>>>(g->SG);
-      if (const cudaError_t e = cudaGetLastError())
-        rc = group_fail(g, B200CONV_ECUDA, std::string("group send launch: ") + cudaGetErrorString(e));
-#endif
-      g->launches++;
-      k = 0;
-    }
-  }
+  if (!rc) rc = group_chain_sends(g);
   if (!rc) rc = group_launch_classes(g);
   const unsigned int want = g->epoch + 1;
-  for (size_t i = 0, k = 0, done = 0; i < n && !rc; ++i) {
-    if (g->prepared[i]) { g->WG.p[k++] = g->wp[i]; ++done; }
-    if (k == (size_t)pc::kChainGroupMax || (k && done == shared)) {
-      g->WG.n = (int)k;
-      const bool last = done == shared;
-      g->WG.done_flag = last ? g->flag_dev : nullptr;
-      g->WG.done_val = want;
-      g->WG.ticket = g->ticket;
-#if defined(PC_EMULATE)
-      pc::emu_chain_wet_group(g->WG);
-#else
-      pc::k_chain_wet_group<<<dim3(wet_blocks, (unsigned)k), 256, 0, g->st>>>(g->WG);
-      if (const cudaError_t e = cudaGetLastError())
-        rc = group_fail(g, B200CONV_ECUDA, std::string("group wet launch: ") + cudaGetErrorString(e));
-#endif
-      g->launches++;
-      k = 0;
-      if (last) { if (!rc) g->epoch = want; break; }
-    }
+  if (!rc && shared) {
+    rc = group_chain_wets(g, g->flag_dev, want);
+    if (!rc) g->epoch = want;
   }
   group_commit(g, waited, &rc);
   // every other member on its own, while the shared launches run
   for (size_t i = 0; i < n && !rc; ++i)
-    if (!g->nc[i])
+    if (!g->nc[i] && !g->lshare[i])
       if (int mrc = b200conv_chain_process(g->m[i], dry[i], ysend ? ysend[i] : nullptr, yrev ? yrev[i] : nullptr, out[i],
                                            len))
         rc = group_member_fail(g, i, mrc);
@@ -3996,6 +4178,34 @@ int b200conv_group_set_member(b200conv_group_t* g, int index, b200conv_t* h) {
   g->m[index] = h;
   return B200CONV_OK;
 }
+
+// Every member is checked against b200conv_set_latency's rules before any changes; then each is switched (and cleared)
+// in member order.  samples == 0 switches back only the members in fixed-latency mode.
+int b200conv_group_set_latency(b200conv_group_t* g, size_t samples) {
+  if (!g) return B200CONV_EINVAL;
+  const size_t n = g->m.size();
+  for (size_t i = 0; i < n; ++i) {
+    const b200conv* h = g->m[i];
+    const std::string who = "member " + std::to_string(i) + ": ";
+    if (h->sticky_cuda_error) return group_member_fail(g, i, B200CONV_ECUDA);
+    if (!samples && !h->lat_D) continue;
+    if (h->stages.empty()) return group_fail(g, B200CONV_ESTATE, who + "no impulse response loaded");
+    if (h->cfg.shard_count > 1) return group_fail(g, B200CONV_ESTATE, who + "fixed-latency mode needs an unsharded handle");
+    if (h->p2p_on || h->p2p_tail) return group_fail(g, B200CONV_ESTATE, who + "the slot exchange is attached");
+    if (h->swap_peer) return group_fail(g, B200CONV_ESTATE, who + "an IR hot swap is pending");
+    const size_t B0 = (size_t)h->stages[0].B;
+    if (samples != 0 && (samples % B0 != 0 || samples > 16 * B0))
+      return group_fail(g, B200CONV_EINVAL, who + "the latency must be a multiple of the head block, at most 16 head blocks");
+  }
+  for (size_t i = 0; i < n; ++i) {
+    if (!samples && !g->m[i]->lat_D) continue;
+    if (int rc = b200conv_set_latency(g->m[i], samples)) return group_member_fail(g, i, rc);
+  }
+  g->lat_D = samples;
+  return B200CONV_OK;
+}
+
+size_t b200conv_group_latency(const b200conv_group_t* g) { return g ? g->lat_D : 0; }
 
 // The chain on the caller's device buffers: the pieces of b200conv_chain_process without staging copies or a
 // synchronise between them.  Pieces of at least kChainWideMin samples run the whole-GPU send form.

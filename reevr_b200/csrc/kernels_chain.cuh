@@ -221,8 +221,9 @@ PC_HD void chain_wet_xfade_sample(const ChainWetParams& P, long long i) {
 }
 
 // The chain calls of up to kChainGroupMax handles in one send and one wet launch (b200conv_chain_group_process),
-// passed by value like RtGroupParams (kernels_rt.cuh).  Every member's wet parameters carry no completion word of
-// their own: the wet launch raises the group's.
+// passed by value like RtGroupParams (kernels_rt.cuh).  In a zero-latency group call the members' wet parameters carry
+// no completion word of their own: the wet launch raises the group's.  In a fixed-latency group call each member's
+// carries its ring word and ticket, and the launch has no group word.
 constexpr int kChainGroupMax = 32;
 struct ChainSendGroupParams {
   int n;
@@ -498,12 +499,17 @@ static __global__ void k_chain_wet_xfade(ChainWetParams P) {
 
 // The wet mix of up to kChainGroupMax handles' chain calls (b200conv_chain_group_process): grid (blocks of 256
 // samples, n), row i of the grid mixes G.p[i] as k_chain_wet would.  The CTA that draws the last ticket of the whole
-// grid raises the group's one completion word (none if G.done_flag is nullptr).
+// grid raises the group's one completion word.  Without one (G.done_flag nullptr), each row whose G.p[i].done_flag is
+// set raises that word once all gridDim.x CTAs of the row have stored (fixed-latency group steps: every member's ring
+// word carries its own sequence value); every CTA of the row counts, also those past a shorter row's n.
 static __global__ void __launch_bounds__(256) k_chain_wet_group(const __grid_constant__ ChainWetGroupParams G) {
   const ChainWetParams& P = G.p[blockIdx.y];
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < P.n) chain_wet_sample(P, i);
-  if (!G.done_flag) return;
+  if (!G.done_flag) {
+    chain_wet_done(P);
+    return;
+  }
   __threadfence_system();
   __syncthreads();
   if (threadIdx.x == 0 && atomicAdd(G.ticket, 1u) == gridDim.x * gridDim.y - 1) {
@@ -1257,7 +1263,10 @@ inline void emu_chain_send_group(const ChainSendGroupParams& G, int T) {
   for (int i = 0; i < G.n; ++i) emu_chain_send(G.p[i], T);
 }
 inline void emu_chain_wet_group(const ChainWetGroupParams& G) {
-  for (int i = 0; i < G.n; ++i) emu_chain_wet(G.p[i]);
+  for (int i = 0; i < G.n; ++i) {
+    for (long long j = 0; j < G.p[i].n; ++j) chain_wet_sample(G.p[i], j);
+    if (!G.done_flag && G.p[i].done_flag) *G.p[i].done_flag = G.p[i].done_val;
+  }
   if (G.done_flag) *G.done_flag = G.done_val;
 }
 #endif
