@@ -1425,20 +1425,20 @@ int launch_mix(b200conv* h, const float* in, size_t in_stride, float* out, size_
 }
 
 // ---- one launch group: n <= Lmax samples, device-resident ------------------------------------
-int compact_timeline(b200conv* h, Stage& s) {
+int compact_timeline(b200conv* h, Stage& s, cudaStream_t st) {
   const int C = h->C, B = s.B;
   const size_t bytes = (size_t)s.hist * B * sizeof(float2);
   for (int c = 0; c < C; ++c) {
     float2* base = s.X + (size_t)c * s.R * B;
-    CU_CHECK(h, cudaMemcpyAsync(base, base + (size_t)(s.head - s.hist) * B, bytes, cudaMemcpyDeviceToDevice, h->s_launch));
+    CU_CHECK(h, cudaMemcpyAsync(base, base + (size_t)(s.head - s.hist) * B, bytes, cudaMemcpyDeviceToDevice, st));
   }
   s.head = s.hist;
   return 0;
 }
 
-// room for nb more X rows from the open block on (plus the sweeps' slack rows)
-int ensure_rows(b200conv* h, Stage& s, int nb) {
-  return s.head + nb + kMaxTT > s.R ? compact_timeline(h, s) : 0;
+// room for nb more X rows from the open block on (plus the sweeps' slack rows); a compaction is queued on st
+int ensure_rows(b200conv* h, Stage& s, int nb, cudaStream_t st) {
+  return s.head + nb + kMaxTT > s.R ? compact_timeline(h, s, st) : 0;
 }
 
 // How a Stage maps onto the kernels' parameter blocks.  The sweep of `nblocks` blocks from the open one on writes Y
@@ -1788,7 +1788,7 @@ int run_tail_stages(b200conv* h, const float* in_dev, size_t in_stride, size_t n
     Intake it;
     if (int rc = intake_begin(h, s, in_dev, in_stride, n, &it)) return rc;
     if (it.complete > 0) {
-      if (int rc = ensure_rows(h, s, it.complete)) return rc;
+      if (int rc = ensure_rows(h, s, it.complete, h->s_launch)) return rc;
       const pc::FwdParams fp = fwd_params(h, s, it.src, it.src_stride, (long long)it.total, it.complete, it.direct);
       if (int rc = launch_fwd(h, fp, C)) return rc;
       for (int j = 0; j < it.complete; ++j) {
@@ -1817,7 +1817,7 @@ int run_group_p2p(b200conv* h, const float* in_dev, size_t in_stride, float* out
   const int nb = complete + (it.partial > 0 ? 1 : 0);
   const int yb = s.ybuf;
   const int per = (nb + G - 1) / G;
-  if (int rc = ensure_rows(h, s, nb)) return rc;
+  if (int rc = ensure_rows(h, s, nb, h->s_launch)) return rc;
   // (routing is refused on this path: the input map stays unused)
   const pc::FwdParams fp = fwd_params(h, s, it.src, it.src_stride, (long long)it.total, nb, it.direct);
   if (int rc = launch_fwd(h, fp, C)) return rc;
@@ -1908,7 +1908,7 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
     TcDirect td{};
     long long yc_stride = 0;
     if (nb > 0) {
-      if (int rc = ensure_rows(h, s, nb)) return rc;
+      if (int rc = ensure_rows(h, s, nb, h->s_launch)) return rc;
       // overlap state after a forward-FFT-only advance (time-slice sharding): Y row 0 must become
       // sum_p H[p] X[head-1-p], the spectrum of the block in front of this group — its input spectra are in the
       // timeline, so the sweep simply starts one block early and writes that block as row 0
@@ -2007,7 +2007,7 @@ int advance_fft_only(b200conv* h, const float* in_dev, size_t in_stride, long lo
   const int C = h->C, B = s.B;
   for (long long done = 0; done < nblocks;) {
     const int nb = (int)std::min<long long>(nblocks - done, s.Tcap);
-    if (int rc = ensure_rows(h, s, nb)) return rc;
+    if (int rc = ensure_rows(h, s, nb, h->s_launch)) return rc;
     const pc::FwdParams fp = fwd_params(h, s, in_dev + (size_t)done * B, in_stride, (long long)nb * B, nb, false);
     if (int rc = launch_fwd(h, fp, C)) return rc;
     s.head += nb;
@@ -2063,7 +2063,7 @@ int drain_tail(b200conv* h) {
 // ONE completed block of a stage >= 1 (its samples are in s.inbuf), everything on h->s_launch: forward FFT into the
 // timeline, streaming sweep, inverse FFT into the stage's look-ahead ring (TwoStageFFTConvolver.cpp:201-222)
 int run_tail_block(b200conv* h, Stage& s) {
-  if (int rc = ensure_rows(h, s, 1)) return rc;
+  if (int rc = ensure_rows(h, s, 1, h->s_launch)) return rc;
   const pc::FwdParams fp = fwd_params(h, s, s.inbuf, s.in_stride, s.B, 1, false);
   if (int rc = launch_fwd(h, fp, h->C)) return rc;
   // on rank 0 of a tail-sharded handle the other ranks' partial spectra join here
@@ -2158,8 +2158,8 @@ bool rt_set_attr() {
 
 // A real-time call (rt_cluster_ctas() > 0) runs as prepare, launch, commit; b200conv_group_process prepares several
 // handles, launches them together and commits them.  `in` / `out` are device-accessible (pinned host or device memory).
-// Prepare: the waits for tail outputs the call needs (queued on `st`, the stream the launch goes to; *waited is set if
-// there was one), room in the timeline, and the call's parameters.  Split mode (nc < 0) is set up by rt_call.
+// Prepare: the waits for tail outputs the call needs and room in the timeline, both queued on `st`, the stream the launch
+// goes to (*waited is set if there was a wait), and the call's parameters.  Split mode (nc < 0) is set up by rt_call.
 int rt_prepare(b200conv* h, int nc, const float* in, size_t in_stride, float* out, size_t out_stride, size_t len,
                cudaStream_t st, pc::RtParams& P, bool* waited) {
   const int C = h->C;
@@ -2178,7 +2178,7 @@ int rt_prepare(b200conv* h, int nc, const float* in, size_t in_stride, float* ou
   }
   // a call that crosses the block boundary: len1 samples complete the open block, the other r start the next one
   const int len1 = std::min((int)len, M - s0.fill), r = (int)len - len1;
-  if (int rc = ensure_rows(h, s0, r ? 2 : 1)) return rc;
+  if (int rc = ensure_rows(h, s0, r ? 2 : 1, st)) return rc;
   P = pc::RtParams{};
   P.M = M; P.C = C; P.NC = nc; P.P = s0.P;
   P.len = (int)len; P.nseg = r ? 2 : 1;
@@ -2292,6 +2292,19 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
   }
   bool recorded = false;
   return rt_commit(h, P, h->ev_rt, h->s_main, &recorded);
+}
+
+// Waits until the pinned completion word *f reached `want`: spins, and after 20 ms synchronises st, the stream that
+// holds the work raising it, so that a device error is reported from there.  False if the word is still not raised
+// then, with *e the synchronise's error (cudaSuccess: st completed without raising it).
+bool wait_word(const volatile unsigned int* f, unsigned int want, cudaStream_t st, cudaError_t* e) {
+  const auto t0 = std::chrono::steady_clock::now();
+  for (unsigned spins = 1; (int)(*f - want) < 0; ++spins)
+    if ((spins & 0x3ff) == 0 && std::chrono::steady_clock::now() - t0 > std::chrono::milliseconds(20)) {
+      *e = cudaStreamSynchronize(st);
+      return !*e && (int)(*f - want) >= 0;
+    }
+  return true;
 }
 
 // b200conv_reset / b200conv_destroy of either handle of a pending IR hot swap: the live handle continues alone
@@ -2642,17 +2655,11 @@ static int process_impl(b200conv_t* h, const float* const* in, float* const* out
       if (int rc = rt_call(h, nc, h->hpin_in_dev, len, h->hpin_out_dev, len, len, h->hflag_dev,
                            h->hflag_dev ? ++h->flag_epoch : 0)) return rc;
       // wait for the kernel's completion word (set after all output stores) instead of the driver's stream
-      // synchronise; if it does not show up within 20 ms, fall back to the synchronise (and its error report)
-      bool done = false;
-      if (h->hflag_dev) {
-        volatile unsigned int* f = h->hflag;
-        const unsigned int want = h->flag_epoch;
-        const auto t0 = std::chrono::steady_clock::now();
-        for (unsigned spins = 0; !(done = ((int)(*f - want) >= 0)); ++spins)
-          if ((spins & 0x3ff) == 0x3ff &&
-              std::chrono::steady_clock::now() - t0 > std::chrono::milliseconds(20)) break;
-      }
-      if (!done) CU_CHECK(h, cudaStreamSynchronize(h->s_main));
+      // synchronise; wait_word falls back to the synchronise (and its error report)
+      cudaError_t e = cudaSuccess;
+      if (!h->hflag_dev) e = cudaStreamSynchronize(h->s_main);
+      else wait_word(h->hflag, h->flag_epoch, h->s_main, &e);
+      if (e) return cuda_fail(h, e, "cudaStreamSynchronize(h->s_main)");
       h->main_unsynced = false;           // the kernel was the last work on s_main
       if (out)
         for (int c = 0; c < Cout; ++c) std::memcpy(out[c], h->hpin_out + (size_t)c * len, len * sizeof(float));
@@ -2728,20 +2735,16 @@ static int launch_seq_flag(b200conv_t* h, unsigned int* flag, unsigned int v, cu
   return 0;
 }
 
-// Waits until ring r's sequence word reached `want`: spins, and after 20 ms synchronises the stream of the ring's last
-// step (every earlier step is ordered before it; a device error is reported from there).  *waited: a wait was needed.
+// Waits until ring r's sequence word reached `want`, with the stream of the ring's last step behind wait_word's
+// fallback (every earlier step is ordered before it).  *waited: a wait was needed.
 static int lat_wait(b200conv_t* h, LatRing* r, unsigned int want, bool* waited) {
-  volatile unsigned int* f = r->word;
+  const volatile unsigned int* f = r->word;
   if ((int)(*f - want) >= 0) return 0;
   *waited = true;
-  const auto t0 = std::chrono::steady_clock::now();
-  for (unsigned spins = 1; (int)(*f - want) < 0; ++spins)
-    if ((spins & 0x3ff) == 0 && std::chrono::steady_clock::now() - t0 > std::chrono::milliseconds(20)) {
-      CU_CHECK(h, cudaStreamSynchronize(r->last_st));
-      if ((int)(*f - want) < 0) return fail(h, B200CONV_ECUDA, "a fixed-latency step did not raise its completion word");
-      break;
-    }
-  return 0;
+  cudaError_t e = cudaSuccess;
+  if (wait_word(f, want, r->last_st, &e)) return 0;
+  if (e) return cuda_fail(h, e, "cudaStreamSynchronize(r->last_st)");
+  return fail(h, B200CONV_ECUDA, "a fixed-latency step did not raise its completion word");
 }
 
 // A call in fixed-latency mode runs in passes of at most r->piece samples.  Input half of a pass of n samples, samples
@@ -2854,252 +2857,6 @@ int b200conv_process(b200conv_t* h, const float* const* in, float* const* out, s
 int b200conv_prime(b200conv_t* h, const float* const* in, size_t len) {
   if (h && h->lat_D) return fail(h, B200CONV_ESTATE, "b200conv_prime is not available in fixed-latency mode");
   return process_impl(h, in, nullptr, len);
-}
-
-// ---- groups (b200conv_group_process) ---------------------------------------------------------------------------------
-// The real-time calls of the qualifying members run as one k_rt_group launch per shape class on the group's own
-// high-priority stream: prepare every member, launch, commit every member.  Event rules:
-//  - a member's tail-output waits (rt_prepare) go on the group stream;
-//  - a member whose s_main may hold unsynchronised work (main_unsynced) orders the group stream behind it once;
-//  - if either happened, or a member completes a tail block, the group records ONE event after its launches: the
-//    s_tail of every member that completes a tail block waits on it before run_tail_block, and every prepared member
-//    keeps it in grp_ev, so that its next own call orders s_main and s_post behind it (set_device).
-// A Stage's job_waited therefore means "ordered before this handle's next head-stage work", through s_main or through
-// the group stream and grp_ev.  In steady state (no tail block completes, nothing unsynchronised) a group call makes
-// no event operation at all: one launch per shape class, then one spin per member on its completion word.
-struct b200conv_group {
-  std::vector<b200conv*> m;
-  int device = 0;
-  std::string err;
-  cudaStream_t st = nullptr;
-  cudaEvent_t ev = nullptr;
-  unsigned long long launches = 0;
-  // per-call scratch, sized by create: a group call allocates nothing
-  std::vector<pc::RtParams> P;
-  std::vector<int> nc;                   // cluster width of a qualifying member, 0: it runs its own b200conv_process
-  std::vector<char> prepared, launched;
-  pc::RtGroupParams G;
-  // b200conv_chain_group_process: the shared members' send / wet parameters, the tables of one launch, the group's
-  // pinned completion word (+ its device-side address) and the wet launch's ticket word on the device
-  std::vector<pc::ChainSendParams> sp;
-  std::vector<pc::ChainWetParams> wp;
-  pc::ChainSendGroupParams SG;
-  pc::ChainWetGroupParams WG;
-  unsigned int* flag = nullptr;
-  unsigned int* flag_dev = nullptr;
-  unsigned int epoch = 0;
-  unsigned int* ticket = nullptr;
-  // fixed-latency group calls (b200conv_group_set_latency): the group's latency (0: none); per member whether it
-  // shares the call's steps, the ring position its current pass began at and whether the call waited for its ring
-  size_t lat_D = 0;
-  std::vector<char> lshare, lwaited;
-  std::vector<long long> lp0;
-};
-
-static int group_fail(b200conv_group* g, int code, const std::string& msg) { g->err = msg; return code; }
-static int group_member_fail(b200conv_group* g, size_t i, int code) {
-  g->err = "member " + std::to_string(i) + ": " + g->m[i]->err;
-  return code;
-}
-
-// cluster width of a member's call when it can share the group's launch, else 0
-static int group_ctas(const b200conv* h, size_t len) {
-  if (h->cfg.shard_count != 1 || h->lat_D || h->stages.empty() || len > h->hpin_cap || !h->hpin_in_dev ||
-      !h->hpin_out_dev || !h->hflag_dev)
-    return 0;
-  return std::max(rt_cluster_ctas(h, len), 0);
-}
-
-b200conv_group_t* b200conv_group_create(b200conv_t* const* members, int n) {
-  if (!members || n < 1 || n > 64) return nullptr;
-  for (int i = 0; i < n; ++i) {
-    if (!members[i] || members[i]->cfg.device != members[0]->cfg.device) return nullptr;
-    for (int j = 0; j < i; ++j)
-      if (members[j] == members[i]) return nullptr;
-  }
-  b200conv_group* g = new (std::nothrow) b200conv_group();
-  if (!g) return nullptr;
-  try {
-    g->m.assign(members, members + n);
-    g->P.resize(n); g->nc.resize(n); g->prepared.resize(n); g->launched.resize(n); g->sp.resize(n); g->wp.resize(n);
-    g->lshare.resize(n); g->lwaited.resize(n); g->lp0.resize(n);
-  } catch (...) {
-    delete g;
-    return nullptr;
-  }
-  g->device = members[0]->cfg.device;
-  int lo = 0, hi = 0;
-  bool ok = cudaSetDevice(g->device) == cudaSuccess && cudaDeviceGetStreamPriorityRange(&lo, &hi) == cudaSuccess;
-  ok = ok && cudaStreamCreateWithPriority(&g->st, cudaStreamNonBlocking, hi) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&g->ev, cudaEventDisableTiming) == cudaSuccess;
-  ok = ok && cudaMallocHost((void**)&g->flag, 64) == cudaSuccess;
-  if (ok) *g->flag = 0;
-#if defined(PC_EMULATE)
-  g->flag_dev = g->flag;
-#else
-  ok = ok && cudaHostGetDevicePointer((void**)&g->flag_dev, g->flag, 0) == cudaSuccess;
-#endif
-  ok = ok && cudaMalloc(&g->ticket, sizeof(unsigned int)) == cudaSuccess;
-  ok = ok && cudaMemsetAsync(g->ticket, 0, sizeof(unsigned int), g->st) == cudaSuccess;
-  if (!ok) {
-    cudaGetLastError();
-    b200conv_group_destroy(g);
-    return nullptr;
-  }
-  return g;
-}
-
-void b200conv_group_destroy(b200conv_group_t* g) {
-  if (!g) return;
-  cudaSetDevice(g->device);
-  if (g->st) cudaStreamSynchronize(g->st);
-  for (b200conv* h : g->m) {
-    if (h->grp_ev == g->ev) h->grp_ev = nullptr;        // everything the event covers has completed
-    for (LatRing* r : {h->lat, h->c_lat})                // ... and every step the group stream held
-      if (r && r->last_st == g->st) r->last_st = h->s_main;
-  }
-  if (g->ev) cudaEventDestroy(g->ev);
-  if (g->st) cudaStreamDestroy(g->st);
-  if (g->flag) cudaFreeHost(g->flag);
-  if (g->ticket) cudaFree(g->ticket);
-  delete g;
-}
-
-const char* b200conv_group_last_error(const b200conv_group_t* g) { return g ? g->err.c_str() : "null group"; }
-
-unsigned long long b200conv_group_launch_count(const b200conv_group_t* g) { return g ? g->launches : 0; }
-
-// The prepared members' clusters: one k_rt_group launch per shape class (M, C, NC) and kRtGroupMax members, in
-// member order within a class, on the group stream
-static int group_launch_classes(b200conv_group* g) {
-  const size_t n = g->m.size();
-  for (size_t i = 0; i < n; ++i) {
-    if (!g->prepared[i] || g->launched[i]) continue;
-    const pc::RtParams& A = g->P[i];
-    size_t idx[pc::kRtGroupMax];
-    int k = 0;
-    for (size_t j = i; j < n && k < pc::kRtGroupMax; ++j) {
-      const pc::RtParams& B = g->P[j];
-      if (g->prepared[j] && !g->launched[j] && B.M == A.M && B.C == A.C && B.NC == A.NC) {
-        g->G.p[k] = B;
-        idx[k++] = j;
-      }
-    }
-    g->G.n = k;
-#if defined(PC_EMULATE)
-    pc::emu_rt_group(g->G);
-#else
-    if (const cudaError_t e = rt_launch(g->G, A.M, A.C, A.NC, g->st)) {
-      cudaGetLastError();
-      return group_fail(g, B200CONV_ECUDA, std::string("group launch: ") + cudaGetErrorString(e));
-    }
-#endif
-    g->launches++;
-    for (int j = 0; j < k; ++j) g->launched[idx[j]] = 1;
-  }
-  return 0;
-}
-
-// Commit: head bookkeeping and the tail blocks the launched calls complete, behind the group's event (recorded now if
-// the prepare queued a wait); every prepared member keeps the event for its next own call.  *rc keeps the first error.
-static void group_commit(b200conv_group* g, bool waited, int* rc) {
-  const size_t n = g->m.size();
-  bool recorded = false;
-  if (waited) {
-    if (cudaEventRecord(g->ev, g->st) != cudaSuccess) {
-      cudaGetLastError();
-      if (!*rc) *rc = group_fail(g, B200CONV_ECUDA, "group: event record failed");
-    } else {
-      recorded = true;
-    }
-  }
-  for (size_t i = 0; i < n; ++i) {
-    if (!g->launched[i]) continue;
-    if (int crc = rt_commit(g->m[i], g->P[i], g->ev, g->st, &recorded))
-      if (!*rc) *rc = group_member_fail(g, i, crc);
-  }
-  if (recorded)
-    for (size_t i = 0; i < n; ++i)
-      if (g->prepared[i]) g->m[i]->grp_ev = g->ev;
-}
-
-static int group_lat_passes(b200conv_group* g, const float* const* const* in, const float* const* ysend,
-                            const float* const* yrev, float* const* const* out, size_t len, bool chain);
-
-int b200conv_group_process(b200conv_group_t* g, const float* const* const* in, float* const* const* out, size_t len) {
-  if (!g) return B200CONV_EINVAL;
-  if (len == 0) return B200CONV_OK;
-  if (!in || !out) return group_fail(g, B200CONV_EINVAL, "null buffer");
-  const size_t n = g->m.size();
-  // every member's arguments before anything is enqueued: a refused call advances no member
-  for (size_t i = 0; i < n; ++i) {
-    const b200conv* h = g->m[i];
-    if (h->sticky_cuda_error) return group_member_fail(g, i, B200CONV_ECUDA);
-    if (!in[i] || !out[i]) return group_fail(g, B200CONV_EINVAL, "null buffer of member " + std::to_string(i));
-    if (h->lat_D)
-      for (int c = 0; c < (h->route_on ? h->n_in : h->C); ++c)
-        if (!in[i][c]) return group_fail(g, B200CONV_EINVAL, "null buffer of member " + std::to_string(i));
-  }
-  if (cudaSetDevice(g->device) != cudaSuccess) {
-    cudaGetLastError();
-    return group_fail(g, B200CONV_ECUDA, "cudaSetDevice failed");
-  }
-  // the members at the group's fixed latency first, in shared steps
-  int rc = group_lat_passes(g, in, nullptr, nullptr, out, len, false);
-  bool waited = false;
-  // prepare: inputs into the pinned staging, the waits each call needs, its parameters
-  for (size_t i = 0; i < n; ++i) {
-    b200conv* h = g->m[i];
-    g->prepared[i] = g->launched[i] = 0;
-    g->nc[i] = group_ctas(h, len);
-    if (!g->nc[i] || rc) continue;
-    if (h->main_unsynced) {
-      cudaError_t e = cudaEventRecord(h->ev_rt, h->s_main);
-      if (e == cudaSuccess) e = cudaStreamWaitEvent(g->st, h->ev_rt, 0);
-      if (e != cudaSuccess) {
-        rc = group_member_fail(g, i, cuda_fail(h, e, "group: ordering behind the member's stream"));
-        continue;
-      }
-      h->main_unsynced = false;
-      waited = true;
-    }
-    const int Cin = h->route_on ? h->n_in : h->C;
-    for (int c = 0; c < Cin; ++c) std::memcpy(h->hpin_in + (size_t)c * len, in[i][c], len * sizeof(float));
-    h->s_launch = g->st;                   // a timeline compaction goes to the group stream, ahead of the launch
-    const int prc = rt_prepare(h, g->nc[i], h->hpin_in_dev, len, h->hpin_out_dev, len, len, g->st, g->P[i], &waited);
-    h->s_launch = h->s_main;
-    g->prepared[i] = 1;                    // waits may have been queued even if it failed
-    if (prc) { rc = group_member_fail(g, i, prc); continue; }
-    g->P[i].done_flag = h->hflag_dev;
-    g->P[i].done_val = ++h->flag_epoch;
-  }
-  if (!rc) rc = group_launch_classes(g);
-  group_commit(g, waited, &rc);
-  // every other member on its own, while the shared launches run
-  for (size_t i = 0; i < n && !rc; ++i)
-    if (!g->nc[i] && !g->lshare[i])
-      if (int mrc = b200conv_process(g->m[i], in[i], out[i], len)) rc = group_member_fail(g, i, mrc);
-  // wait for each launched member's completion word; if one does not show up within 20 ms, synchronise the group
-  // stream once (and report its error)
-  const auto t0 = std::chrono::steady_clock::now();
-  bool synced = false;
-  for (size_t i = 0; i < n; ++i) {
-    if (!g->launched[i]) continue;
-    b200conv* h = g->m[i];
-    volatile unsigned int* f = h->hflag;
-    const unsigned int want = g->P[i].done_val;
-    for (unsigned spins = 0; !synced && (int)(*f - want) < 0; ++spins)
-      if ((spins & 0x3ff) == 0x3ff && std::chrono::steady_clock::now() - t0 > std::chrono::milliseconds(20)) {
-        if (const cudaError_t e = cudaStreamSynchronize(g->st)) {
-          cudaGetLastError();
-          return group_fail(g, B200CONV_ECUDA, std::string("group stream: ") + cudaGetErrorString(e));
-        }
-        synced = true;
-      }
-    const int Cout = h->route_on ? h->n_out : h->C;
-    for (int c = 0; c < Cout; ++c) std::memcpy(out[i][c], h->hpin_out + (size_t)c * len, len * sizeof(float));
-  }
-  return rc;
 }
 
 int b200conv_process_device_sliced(b200conv_t* h, const float* in_dev, size_t in_stride, float* out_dev, size_t out_stride,
@@ -3866,347 +3623,6 @@ int b200conv_chain_process(b200conv_t* h, const float* const* dry, const float* 
   return B200CONV_OK;
 }
 
-// The chain calls of a group (b200conv_chain_group_process).  A member shares the group's launches when
-// b200conv_chain_process would run its call as one zero-copy piece through one cluster launch, and it can share a
-// k_rt_group launch: a chain, no fixed latency, no pending hot swap, and group_ctas > 0.  Its width, else 0.
-static int chain_group_ctas(const b200conv* h, size_t len) {
-  if (!h->chain_on || h->lat_D || h->swap_peer || h->stages.empty() || !h->c_hpin_dev || !h->opt_rt ||
-      len > h->Lmax - h->stages[0].B)
-    return 0;
-  return group_ctas(h, len);
-}
-
-// The sends of the prepared members: one k_chain_send_group per send width and kChainGroupMax members, in member order
-static int group_chain_sends(b200conv_group* g) {
-  const size_t n = g->m.size();
-  bool sent[64] = {};                    // b200conv_group_create admits at most 64 members
-  for (size_t i = 0; i < n; ++i) {
-    if (!g->prepared[i] || sent[i]) continue;
-    const int T = chain_send_threads((size_t)g->sp[i].n);
-    int k = 0;
-    for (size_t j = i; j < n && k < pc::kChainGroupMax; ++j)
-      if (g->prepared[j] && !sent[j] && chain_send_threads((size_t)g->sp[j].n) == T) {
-        g->SG.p[k++] = g->sp[j];
-        sent[j] = true;
-      }
-    g->SG.n = k;
-#if defined(PC_EMULATE)
-    pc::emu_chain_send_group(g->SG, T);
-#else
-    pc::k_chain_send_group<<<dim3(2, (unsigned)k), T, 0, g->st>>>(g->SG);
-    if (const cudaError_t e = cudaGetLastError())
-      return group_fail(g, B200CONV_ECUDA, std::string("group send launch: ") + cudaGetErrorString(e));
-#endif
-    g->launches++;
-  }
-  return 0;
-}
-
-// The wet mixes of the prepared members: one k_chain_wet_group per kChainGroupMax members, in member order.  The last
-// raises `flag` to `want`; with flag nullptr every row raises its own member's word instead (fixed-latency steps).
-static int group_chain_wets(b200conv_group* g, unsigned int* flag, unsigned int want) {
-  const size_t n = g->m.size();
-  size_t left = 0;
-  for (size_t i = 0; i < n; ++i) left += g->prepared[i] ? 1 : 0;
-  for (size_t i = 0, k = 0; i < n; ++i) {
-    if (g->prepared[i]) { g->WG.p[k++] = g->wp[i]; --left; }
-    if (k == (size_t)pc::kChainGroupMax || (k && !left)) {
-      unsigned blocks = 0;
-      for (size_t j = 0; j < k; ++j) blocks = std::max(blocks, (unsigned)((g->WG.p[j].n + 255) / 256));
-      g->WG.n = (int)k;
-      g->WG.done_flag = left ? nullptr : flag;
-      g->WG.done_val = want;
-      g->WG.ticket = g->ticket;
-#if defined(PC_EMULATE)
-      pc::emu_chain_wet_group(g->WG);
-#else
-      pc::k_chain_wet_group<<<dim3(blocks, (unsigned)k), 256, 0, g->st>>>(g->WG);
-      if (const cudaError_t e = cudaGetLastError())
-        return group_fail(g, B200CONV_ECUDA, std::string("group wet launch: ") + cudaGetErrorString(e));
-#endif
-      g->launches++;
-      k = 0;
-    }
-  }
-  return 0;
-}
-
-// ---- fixed-latency groups (b200conv_group_set_latency) ---------------------------------------------------------------
-// A member shares the steps of a group call when its latency is the group's and each of its steps would be one cluster
-// launch: lat_step's rt_call path, or for the chain chain_convolve's, with chain rings and no pending hot swap.  Its
-// cluster width, else 0.
-static int group_lat_ctas(const b200conv_group* g, const b200conv* h, bool chain) {
-  if (!g->lat_D || h->lat_D != g->lat_D || h->cfg.shard_count != 1 || h->stages.empty()) return 0;
-  if (chain ? (!h->chain_on || !h->c_lat || h->swap_peer || !h->opt_rt) : (!h->lat || !h->hpin_in_dev || !h->hpin_out_dev))
-    return 0;
-  return std::max(rt_cluster_ctas(h, h->stages[0].B), 0);
-}
-
-// The members that share a group call's fixed-latency steps, walked in passes as lat_run walks one call; a pass is at
-// most the smallest ring piece among them.  Per pass: every sharing member's input half; then rounds, round q holding
-// the q-th step of every member that completes more than q head blocks in the pass, each prepared as lat_step (or the
-// step of chain_process_latency) runs it, with the member's ring word and sequence value, then launched together and
-// committed on the group stream, so that each member's steps stay in order; then every sharing member's output half.
-// The group stream is ordered behind a member's own steps by main_unsynced, as in a zero-latency group call; a call
-// that launched steps records the group's event once, and the members keep it for their next own call (set_device).
-// chain: in / ysend / yrev are the chain's dry / ysend / yrev tables.  Sets lshare for the callers.
-static int group_lat_passes(b200conv_group* g, const float* const* const* in, const float* const* ysend,
-                            const float* const* yrev, float* const* const* out, size_t len, bool chain) {
-  const size_t n = g->m.size();
-  size_t piece = 0;
-  for (size_t i = 0; i < n; ++i) {
-    b200conv* h = g->m[i];
-    g->nc[i] = group_lat_ctas(g, h, chain);
-    g->lshare[i] = g->nc[i] > 0;
-    g->lwaited[i] = 0;
-    if (g->lshare[i]) {
-      const LatRing* r = chain ? h->c_lat : h->lat;
-      piece = piece ? std::min(piece, r->piece) : r->piece;
-    }
-  }
-  int rc = 0;
-  bool stepped = false;
-  for (size_t done = 0; done < len && piece && !rc;) {
-    const long long np = (long long)std::min(len - done, piece);
-    long long rounds = 0;
-    for (size_t i = 0; i < n && !rc; ++i) {
-      if (!g->lshare[i]) continue;
-      b200conv* h = g->m[i];
-      LatRing* r = chain ? h->c_lat : h->lat;
-      const float* rows[4] = {};
-      if (chain) { rows[0] = in[i][0]; rows[1] = in[i][1]; rows[2] = ysend ? ysend[i] : nullptr; rows[3] = yrev ? yrev[i] : nullptr; }
-      bool w = false;
-      g->lp0[i] = r->pos;
-      if (int e = lat_in(h, r, chain ? rows : in[i], chain ? 4 : (h->route_on ? h->n_in : h->C), done, np, &w))
-        rc = group_member_fail(g, i, e);
-      if (w) g->lwaited[i] = 1;
-      const long long B = (long long)r->B;
-      rounds = std::max(rounds, (g->lp0[i] + np) / B - g->lp0[i] / B);
-    }
-    for (long long q = 0; q < rounds && !rc; ++q) {
-      bool waited = false;
-      for (size_t i = 0; i < n; ++i) {
-        g->prepared[i] = g->launched[i] = 0;
-        if (!g->lshare[i] || rc) continue;
-        b200conv* h = g->m[i];
-        LatRing* r = chain ? h->c_lat : h->lat;
-        const long long k = g->lp0[i] / (long long)r->B + q;
-        if (k >= (g->lp0[i] + np) / (long long)r->B) continue;
-        if (h->main_unsynced) {
-          cudaError_t e = cudaEventRecord(h->ev_rt, h->s_main);
-          if (e == cudaSuccess) e = cudaStreamWaitEvent(g->st, h->ev_rt, 0);
-          if (e != cudaSuccess) {
-            rc = group_member_fail(g, i, cuda_fail(h, e, "group: ordering behind the member's stream"));
-            continue;
-          }
-          h->main_unsynced = false;
-          waited = true;
-        }
-        const size_t B = r->B, L = r->len, off = (size_t)(k % (long long)r->nslots) * B;
-        const unsigned int v = ++r->seq;
-        int prc;
-        h->s_launch = g->st;               // a timeline compaction goes to the group stream, ahead of the launches
-        if (chain) {
-          const float* d = r->in_dev + off;
-          chain_piece_params(h, d, d + 2 * L, d + 3 * L, r->out_dev + off, L, L, B, &g->sp[i], &g->wp[i]);
-          g->wp[i].done_flag = r->word_dev; g->wp[i].done_val = v; g->wp[i].ticket = r->ticket;
-          h->route_in_only = true;
-          prc = rt_prepare(h, g->nc[i], h->c_conv_in, h->Lmax, h->dch[0], h->Lmax, B, g->st, g->P[i], &waited);
-          h->route_in_only = false;
-        } else {
-          prc = rt_prepare(h, g->nc[i], r->in_dev + off, L, r->out_dev + off, L, B, g->st, g->P[i], &waited);
-          g->P[i].done_flag = r->word_dev; g->P[i].done_val = v;
-        }
-        h->s_launch = h->s_main;
-        g->prepared[i] = 1;                // waits may have been queued even if it failed
-        if (prc) { rc = group_member_fail(g, i, prc); continue; }
-        r->last_st = g->st;                // lat_wait's fallback synchronises the stream that holds the step
-      }
-      if (!rc && chain) rc = group_chain_sends(g);
-      if (!rc) rc = group_launch_classes(g);
-      if (!rc && chain) rc = group_chain_wets(g, nullptr, 0);
-      group_commit(g, waited, &rc);
-      for (size_t i = 0; i < n && !rc; ++i) {
-        if (!g->launched[i]) continue;
-        LatRing* r = chain ? g->m[i]->c_lat : g->m[i]->lat;
-        const long long k = g->lp0[i] / (long long)r->B + q;
-        r->slot_seq[k % (long long)r->nslots] = chain ? g->wp[i].done_val : g->P[i].done_val;
-        stepped = true;
-      }
-    }
-    for (size_t i = 0; i < n && !rc; ++i) {
-      if (!g->lshare[i]) continue;
-      b200conv* h = g->m[i];
-      bool w = false;
-      if (int e = lat_out(h, chain ? h->c_lat : h->lat, out[i], chain ? 2 : (h->route_on ? h->n_out : h->C), done,
-                          g->lp0[i], np, &w))
-        rc = group_member_fail(g, i, e);
-      if (w) g->lwaited[i] = 1;
-    }
-    done += (size_t)np;
-  }
-  if (stepped) {
-    if (cudaEventRecord(g->ev, g->st) != cudaSuccess) {
-      cudaGetLastError();
-      if (!rc) rc = group_fail(g, B200CONV_ECUDA, "group: event record failed");
-    } else {
-      for (size_t i = 0; i < n; ++i)
-        if (g->lshare[i]) g->m[i]->grp_ev = g->ev;
-    }
-  }
-  for (size_t i = 0; i < n; ++i)                 // a call that waited counts once in the member's latency_waits
-    if (g->lwaited[i]) g->m[i]->lat_waits++;
-  return rc;
-}
-
-int b200conv_chain_group_process(b200conv_group_t* g, const float* const* const* dry, const float* const* ysend,
-                                 const float* const* yrev, float* const* const* out, size_t len) {
-  if (!g) return B200CONV_EINVAL;
-  if (len == 0) return B200CONV_OK;
-  if (!dry || !out) return group_fail(g, B200CONV_EINVAL, "null buffer");
-  const size_t n = g->m.size();
-  // every member's arguments before anything is enqueued: a refused call advances no member
-  for (size_t i = 0; i < n; ++i) {
-    const b200conv* h = g->m[i];
-    if (h->sticky_cuda_error) return group_member_fail(g, i, B200CONV_ECUDA);
-    if (!h->chain_on) return group_fail(g, B200CONV_ESTATE, "member " + std::to_string(i) + " owns no send / wet chain");
-    if (h->stages.empty() || (h->lat_D && !h->c_lat))
-      return group_fail(g, B200CONV_ESTATE, "member " + std::to_string(i) + " has no impulse response or chain rings");
-    if (!dry[i] || !out[i] || !dry[i][0] || !dry[i][1] || !out[i][0] || !out[i][1])
-      return group_fail(g, B200CONV_EINVAL, "null buffer of member " + std::to_string(i));
-  }
-  if (cudaSetDevice(g->device) != cudaSuccess) {
-    cudaGetLastError();
-    return group_fail(g, B200CONV_ECUDA, "cudaSetDevice failed");
-  }
-  int rc = group_lat_passes(g, dry, ysend, yrev, out, len, true);
-  bool waited = false;
-  size_t shared = 0;
-  // prepare: inputs into the chain's pinned staging, the send / wet parameters, the waits the convolver call needs
-  // and its parameters (input: the predelayed send, outputs: the per-convolver rows, as chain_convolve runs it)
-  for (size_t i = 0; i < n; ++i) {
-    b200conv* h = g->m[i];
-    g->prepared[i] = g->launched[i] = 0;
-    g->nc[i] = chain_group_ctas(h, len);
-    if (!g->nc[i] || rc) continue;
-    if (h->main_unsynced) {
-      cudaError_t e = cudaEventRecord(h->ev_rt, h->s_main);
-      if (e == cudaSuccess) e = cudaStreamWaitEvent(g->st, h->ev_rt, 0);
-      if (e != cudaSuccess) {
-        rc = group_member_fail(g, i, cuda_fail(h, e, "group: ordering behind the member's stream"));
-        continue;
-      }
-      h->main_unsynced = false;
-      waited = true;
-    }
-    const size_t cap = h->hpin_cap;
-    std::memcpy(h->c_hpin, dry[i][0], len * sizeof(float));
-    std::memcpy(h->c_hpin + cap, dry[i][1], len * sizeof(float));
-    const float* ys = ysend ? ysend[i] : nullptr;
-    const float* yr = yrev ? yrev[i] : nullptr;
-    if (ys) std::memcpy(h->c_hpin + 2 * cap, ys, len * sizeof(float));
-    if (yr) std::memcpy(h->c_hpin + 3 * cap, yr, len * sizeof(float));
-    float* d = h->c_hpin_dev;
-    chain_piece_params(h, d, ys ? d + 2 * cap : nullptr, yr ? d + 3 * cap : nullptr, d + 4 * cap, cap, cap, len,
-                       &g->sp[i], &g->wp[i]);
-    h->route_in_only = true;
-    h->s_launch = g->st;                   // a timeline compaction goes to the group stream, ahead of the launches
-    const int prc = rt_prepare(h, g->nc[i], h->c_conv_in, h->Lmax, h->dch[0], h->Lmax, len, g->st, g->P[i], &waited);
-    h->s_launch = h->s_main;
-    h->route_in_only = false;
-    g->prepared[i] = 1;                    // waits may have been queued even if it failed
-    if (prc) { rc = group_member_fail(g, i, prc); continue; }
-    ++shared;
-  }
-  // launch: the sends (one per kChainGroupMax members), the convolvers (one per shape class), the wet mixes (one per
-  // kChainGroupMax members, the last of them raises the group's word), all in member order on the group stream
-  if (!rc) rc = group_chain_sends(g);
-  if (!rc) rc = group_launch_classes(g);
-  const unsigned int want = g->epoch + 1;
-  if (!rc && shared) {
-    rc = group_chain_wets(g, g->flag_dev, want);
-    if (!rc) g->epoch = want;
-  }
-  group_commit(g, waited, &rc);
-  // every other member on its own, while the shared launches run
-  for (size_t i = 0; i < n && !rc; ++i)
-    if (!g->nc[i] && !g->lshare[i])
-      if (int mrc = b200conv_chain_process(g->m[i], dry[i], ysend ? ysend[i] : nullptr, yrev ? yrev[i] : nullptr, out[i],
-                                           len))
-        rc = group_member_fail(g, i, mrc);
-  if (!shared || g->epoch != want) return rc;
-  // one completion word for every shared member; if it does not show up within 20 ms, synchronise the group stream
-  // once (and report its error)
-  volatile unsigned int* f = g->flag;
-  const auto t0 = std::chrono::steady_clock::now();
-  for (unsigned spins = 0; (int)(*f - want) < 0; ++spins)
-    if ((spins & 0x3ff) == 0x3ff && std::chrono::steady_clock::now() - t0 > std::chrono::milliseconds(20)) {
-      if (const cudaError_t e = cudaStreamSynchronize(g->st)) {
-        cudaGetLastError();
-        return group_fail(g, B200CONV_ECUDA, std::string("group stream: ") + cudaGetErrorString(e));
-      }
-      break;
-    }
-  for (size_t i = 0; i < n; ++i) {
-    if (!g->launched[i]) continue;
-    const b200conv* h = g->m[i];
-    for (int ch = 0; ch < 2; ++ch) std::memcpy(out[i][ch], h->c_hpin + (4 + ch) * h->hpin_cap, len * sizeof(float));
-  }
-  return rc;
-}
-
-// A completed b200conv_chain_swap moves the chain to the incoming handle: the caller puts it in the outgoing one's
-// place.  The outgoing handle's next own call must still follow the group's event if it holds it.
-int b200conv_group_set_member(b200conv_group_t* g, int index, b200conv_t* h) {
-  if (!g) return B200CONV_EINVAL;
-  if (index < 0 || (size_t)index >= g->m.size()) return group_fail(g, B200CONV_EINVAL, "member index out of range");
-  if (!h) return group_fail(g, B200CONV_EINVAL, "null member");
-  if (h->cfg.device != g->device) return group_fail(g, B200CONV_EINVAL, "the member is on another device");
-  for (size_t j = 0; j < g->m.size(); ++j)
-    if (g->m[j] == h && (int)j != index) return group_fail(g, B200CONV_EINVAL, "the handle is already a member");
-  b200conv* old = g->m[index];
-  if (old != h && old->grp_ev == g->ev) {
-    cudaError_t e = cudaSetDevice(g->device);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(old->s_main, g->ev, 0);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(old->s_post, g->ev, 0);
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      return group_fail(g, B200CONV_ECUDA, std::string("set_member: ") + cudaGetErrorString(e));
-    }
-    old->grp_ev = nullptr;
-  }
-  g->m[index] = h;
-  return B200CONV_OK;
-}
-
-// Every member is checked against b200conv_set_latency's rules before any changes; then each is switched (and cleared)
-// in member order.  samples == 0 switches back only the members in fixed-latency mode.
-int b200conv_group_set_latency(b200conv_group_t* g, size_t samples) {
-  if (!g) return B200CONV_EINVAL;
-  const size_t n = g->m.size();
-  for (size_t i = 0; i < n; ++i) {
-    const b200conv* h = g->m[i];
-    const std::string who = "member " + std::to_string(i) + ": ";
-    if (h->sticky_cuda_error) return group_member_fail(g, i, B200CONV_ECUDA);
-    if (!samples && !h->lat_D) continue;
-    if (h->stages.empty()) return group_fail(g, B200CONV_ESTATE, who + "no impulse response loaded");
-    if (h->cfg.shard_count > 1) return group_fail(g, B200CONV_ESTATE, who + "fixed-latency mode needs an unsharded handle");
-    if (h->p2p_on || h->p2p_tail) return group_fail(g, B200CONV_ESTATE, who + "the slot exchange is attached");
-    if (h->swap_peer) return group_fail(g, B200CONV_ESTATE, who + "an IR hot swap is pending");
-    const size_t B0 = (size_t)h->stages[0].B;
-    if (samples != 0 && (samples % B0 != 0 || samples > 16 * B0))
-      return group_fail(g, B200CONV_EINVAL, who + "the latency must be a multiple of the head block, at most 16 head blocks");
-  }
-  for (size_t i = 0; i < n; ++i) {
-    if (!samples && !g->m[i]->lat_D) continue;
-    if (int rc = b200conv_set_latency(g->m[i], samples)) return group_member_fail(g, i, rc);
-  }
-  g->lat_D = samples;
-  return B200CONV_OK;
-}
-
-size_t b200conv_group_latency(const b200conv_group_t* g) { return g ? g->lat_D : 0; }
-
 // The chain on the caller's device buffers: the pieces of b200conv_chain_process without staging copies or a
 // synchronise between them.  Pieces of at least kChainWideMin samples run the whole-GPU send form.
 int b200conv_chain_process_device(b200conv_t* h, const float* dry_dev, size_t dry_stride, const float* ysend_dev,
@@ -4371,6 +3787,580 @@ int b200conv_chain_swap(b200conv_t* live, b200conv_t* incoming, size_t host_bloc
 }
 
 int b200conv_chain_swap_state(const b200conv_t* h) { return h ? h->swap_state : 0; }
+
+// ---- groups (b200conv_group_process, b200conv_chain_group_process) --------------------------------------------------
+// The real-time calls of the qualifying members run as one k_rt_group launch per shape class on the group's own
+// high-priority stream: prepare every member, launch, commit every member.  Event rules:
+//  - a member's tail-output waits (rt_prepare) go on the group stream;
+//  - a member whose s_main may hold unsynchronised work (main_unsynced) orders the group stream behind it once;
+//  - if either happened, or a member completes a tail block, the group records ONE event after its launches: the
+//    s_tail of every member that completes a tail block waits on it before run_tail_block, and every prepared member
+//    keeps it in grp_ev, so that its next own call orders s_main and s_post behind it (set_device).
+// A Stage's job_waited therefore means "ordered before this handle's next head-stage work", through s_main or through
+// the group stream and grp_ev.  In steady state (no tail block completes, nothing unsynchronised) a group call makes
+// no event operation at all: one launch per shape class, then one spin per member on its completion word.
+
+// A member's part of the step a group call is running
+struct GroupSlot {
+  pc::RtParams P;                    // the convolver call
+  pc::ChainSendParams sp;            // a chain member's send and wet mix
+  pc::ChainWetParams wp;
+  int nc = 0;                        // cluster width of a member that shares the launches, 0: it runs its own call
+  bool prepared = false, launched = false;
+  bool shares_latency = false;       // fixed-latency group calls: the member shares the call's steps,
+  bool waited = false;               // ... the call waited for its ring
+  long long p0 = 0;                  // ... and the ring position its current pass began at
+};
+
+struct b200conv_group {
+  std::vector<b200conv*> m;
+  int device = 0;
+  std::string err;
+  cudaStream_t st = nullptr;
+  cudaEvent_t ev = nullptr;
+  unsigned long long launches = 0;
+  // per-call scratch, sized by create: a group call allocates nothing
+  std::vector<GroupSlot> slot;
+  pc::RtGroupParams G;                   // the tables of one launch
+  pc::ChainSendGroupParams SG;
+  pc::ChainWetGroupParams WG;
+  // b200conv_chain_group_process: the group's pinned completion word (+ its device-side address) and the wet launch's
+  // ticket word on the device
+  unsigned int* flag = nullptr;
+  unsigned int* flag_dev = nullptr;
+  unsigned int epoch = 0;
+  unsigned int* ticket = nullptr;
+  // fixed-latency group calls (b200conv_group_set_latency): the group's latency (0: none)
+  size_t lat_D = 0;
+};
+
+static int group_fail(b200conv_group* g, int code, const std::string& msg) { g->err = msg; return code; }
+static int group_member_fail(b200conv_group* g, size_t i, int code) {
+  g->err = "member " + std::to_string(i) + ": " + g->m[i]->err;
+  return code;
+}
+
+// cluster width of a member's call when it can share the group's launch, else 0
+static int group_ctas(const b200conv* h, size_t len) {
+  if (h->cfg.shard_count != 1 || h->lat_D || h->stages.empty() || len > h->hpin_cap || !h->hpin_in_dev ||
+      !h->hpin_out_dev || !h->hflag_dev)
+    return 0;
+  return std::max(rt_cluster_ctas(h, len), 0);
+}
+
+// The chain calls of a group (b200conv_chain_group_process).  A member shares the group's launches when
+// b200conv_chain_process would run its call as one zero-copy piece through one cluster launch, and it can share a
+// k_rt_group launch: a chain, no fixed latency, no pending hot swap, and group_ctas > 0.  Its width, else 0.
+static int chain_group_ctas(const b200conv* h, size_t len) {
+  if (!h->chain_on || h->lat_D || h->swap_peer || h->stages.empty() || !h->c_hpin_dev || !h->opt_rt ||
+      len > h->Lmax - h->stages[0].B)
+    return 0;
+  return group_ctas(h, len);
+}
+
+// Fixed-latency groups (b200conv_group_set_latency): a member shares the steps of a group call when its latency is the
+// group's and each of its steps would be one cluster launch: lat_step's rt_call path, or for the chain
+// chain_convolve's, with chain rings and no pending hot swap.  Its cluster width, else 0.
+static int group_lat_ctas(const b200conv_group* g, const b200conv* h, bool chain) {
+  if (!g->lat_D || h->lat_D != g->lat_D || h->cfg.shard_count != 1 || h->stages.empty()) return 0;
+  if (chain ? (!h->chain_on || !h->c_lat || h->swap_peer || !h->opt_rt) : (!h->lat || !h->hpin_in_dev || !h->hpin_out_dev))
+    return 0;
+  return std::max(rt_cluster_ctas(h, h->stages[0].B), 0);
+}
+
+b200conv_group_t* b200conv_group_create(b200conv_t* const* members, int n) {
+  if (!members || n < 1 || n > 64) return nullptr;
+  for (int i = 0; i < n; ++i) {
+    if (!members[i] || members[i]->cfg.device != members[0]->cfg.device) return nullptr;
+    for (int j = 0; j < i; ++j)
+      if (members[j] == members[i]) return nullptr;
+  }
+  b200conv_group* g = new (std::nothrow) b200conv_group();
+  if (!g) return nullptr;
+  try {
+    g->m.assign(members, members + n);
+    g->slot.resize(n);
+  } catch (...) {
+    delete g;
+    return nullptr;
+  }
+  g->device = members[0]->cfg.device;
+  int lo = 0, hi = 0;
+  bool ok = cudaSetDevice(g->device) == cudaSuccess && cudaDeviceGetStreamPriorityRange(&lo, &hi) == cudaSuccess;
+  ok = ok && cudaStreamCreateWithPriority(&g->st, cudaStreamNonBlocking, hi) == cudaSuccess;
+  ok = ok && cudaEventCreateWithFlags(&g->ev, cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && cudaMallocHost((void**)&g->flag, 64) == cudaSuccess;
+  if (ok) *g->flag = 0;
+#if defined(PC_EMULATE)
+  g->flag_dev = g->flag;
+#else
+  ok = ok && cudaHostGetDevicePointer((void**)&g->flag_dev, g->flag, 0) == cudaSuccess;
+#endif
+  ok = ok && cudaMalloc(&g->ticket, sizeof(unsigned int)) == cudaSuccess;
+  ok = ok && cudaMemsetAsync(g->ticket, 0, sizeof(unsigned int), g->st) == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    b200conv_group_destroy(g);
+    return nullptr;
+  }
+  return g;
+}
+
+void b200conv_group_destroy(b200conv_group_t* g) {
+  if (!g) return;
+  cudaSetDevice(g->device);
+  if (g->st) cudaStreamSynchronize(g->st);
+  for (b200conv* h : g->m) {
+    if (h->grp_ev == g->ev) h->grp_ev = nullptr;        // everything the event covers has completed
+    for (LatRing* r : {h->lat, h->c_lat})                // ... and every step the group stream held
+      if (r && r->last_st == g->st) r->last_st = h->s_main;
+  }
+  if (g->ev) cudaEventDestroy(g->ev);
+  if (g->st) cudaStreamDestroy(g->st);
+  if (g->flag) cudaFreeHost(g->flag);
+  if (g->ticket) cudaFree(g->ticket);
+  delete g;
+}
+
+const char* b200conv_group_last_error(const b200conv_group_t* g) { return g ? g->err.c_str() : "null group"; }
+
+unsigned long long b200conv_group_launch_count(const b200conv_group_t* g) { return g ? g->launches : 0; }
+
+// A member whose s_main may hold unsynchronised work (main_unsynced) orders the group stream behind it; *waited is set
+static int group_order_behind(b200conv_group* g, size_t i, bool* waited) {
+  b200conv* h = g->m[i];
+  if (!h->main_unsynced) return 0;
+  cudaError_t e = cudaEventRecord(h->ev_rt, h->s_main);
+  if (e == cudaSuccess) e = cudaStreamWaitEvent(g->st, h->ev_rt, 0);
+  if (e != cudaSuccess) return group_member_fail(g, i, cuda_fail(h, e, "group: ordering behind the member's stream"));
+  h->main_unsynced = false;
+  *waited = true;
+  return 0;
+}
+
+// Prepares member i's step of len samples on the group stream (its waits and a timeline compaction go there; *waited is
+// set if there was a wait).  in: the input rows, in_stride apart; for a chain member the dry rows, with the send / rev
+// envelope rows (nullptr: envelope 1).  out: the output rows, out_stride apart.  flag / val: the step's completion word
+// and value, ticket: the wet kernel's ticket word of a chain member (nullptr / 0: none).  A chain member's send and wet
+// come from chain_piece_params, which moves the chain past the step; its convolvers run from c_conv_in into dch[0], as
+// chain_convolve runs them.  The member counts as prepared even if this fails: waits may have been queued.
+static int group_prepare_step(b200conv_group* g, size_t i, bool chain, const float* in, const float* send,
+                              const float* rev, size_t in_stride, float* out, size_t out_stride, size_t len,
+                              unsigned int* flag, unsigned int val, unsigned int* ticket, bool* waited) {
+  b200conv* h = g->m[i];
+  GroupSlot& s = g->slot[i];
+  int rc;
+  if (chain) {
+    chain_piece_params(h, in, send, rev, out, in_stride, out_stride, len, &s.sp, &s.wp);
+    s.wp.done_flag = flag; s.wp.done_val = val; s.wp.ticket = ticket;
+    h->route_in_only = true;
+    rc = rt_prepare(h, s.nc, h->c_conv_in, h->Lmax, h->dch[0], h->Lmax, len, g->st, s.P, waited);
+    h->route_in_only = false;
+  } else {
+    rc = rt_prepare(h, s.nc, in, in_stride, out, out_stride, len, g->st, s.P, waited);
+    s.P.done_flag = flag; s.P.done_val = val;
+  }
+  s.prepared = true;
+  return rc ? group_member_fail(g, i, rc) : 0;
+}
+
+// The prepared members' clusters: one k_rt_group launch per shape class (M, C, NC) and kRtGroupMax members, in
+// member order within a class, on the group stream
+static int group_launch_classes(b200conv_group* g) {
+  const size_t n = g->m.size();
+  for (size_t i = 0; i < n; ++i) {
+    if (!g->slot[i].prepared || g->slot[i].launched) continue;
+    const pc::RtParams& A = g->slot[i].P;
+    size_t idx[pc::kRtGroupMax];
+    int k = 0;
+    for (size_t j = i; j < n && k < pc::kRtGroupMax; ++j) {
+      const GroupSlot& s = g->slot[j];
+      if (s.prepared && !s.launched && s.P.M == A.M && s.P.C == A.C && s.P.NC == A.NC) {
+        g->G.p[k] = s.P;
+        idx[k++] = j;
+      }
+    }
+    g->G.n = k;
+#if defined(PC_EMULATE)
+    pc::emu_rt_group(g->G);
+#else
+    if (const cudaError_t e = rt_launch(g->G, A.M, A.C, A.NC, g->st)) {
+      cudaGetLastError();
+      return group_fail(g, B200CONV_ECUDA, std::string("group launch: ") + cudaGetErrorString(e));
+    }
+#endif
+    g->launches++;
+    for (int j = 0; j < k; ++j) g->slot[idx[j]].launched = true;
+  }
+  return 0;
+}
+
+// The sends of the prepared members: one k_chain_send_group per send width and kChainGroupMax members, in member order
+static int group_chain_sends(b200conv_group* g) {
+  const size_t n = g->m.size();
+  bool sent[64] = {};                    // b200conv_group_create admits at most 64 members
+  for (size_t i = 0; i < n; ++i) {
+    if (!g->slot[i].prepared || sent[i]) continue;
+    const int T = chain_send_threads((size_t)g->slot[i].sp.n);
+    int k = 0;
+    for (size_t j = i; j < n && k < pc::kChainGroupMax; ++j)
+      if (g->slot[j].prepared && !sent[j] && chain_send_threads((size_t)g->slot[j].sp.n) == T) {
+        g->SG.p[k++] = g->slot[j].sp;
+        sent[j] = true;
+      }
+    g->SG.n = k;
+#if defined(PC_EMULATE)
+    pc::emu_chain_send_group(g->SG, T);
+#else
+    pc::k_chain_send_group<<<dim3(2, (unsigned)k), T, 0, g->st>>>(g->SG);
+    if (const cudaError_t e = cudaGetLastError())
+      return group_fail(g, B200CONV_ECUDA, std::string("group send launch: ") + cudaGetErrorString(e));
+#endif
+    g->launches++;
+  }
+  return 0;
+}
+
+// The wet mixes of the prepared members: one k_chain_wet_group per kChainGroupMax members, in member order.  The last
+// raises `flag` to `want`; with flag nullptr every row raises its own member's word instead (fixed-latency steps).
+static int group_chain_wets(b200conv_group* g, unsigned int* flag, unsigned int want) {
+  const size_t n = g->m.size();
+  size_t left = 0;
+  for (size_t i = 0; i < n; ++i) left += g->slot[i].prepared ? 1 : 0;
+  for (size_t i = 0, k = 0; i < n; ++i) {
+    if (g->slot[i].prepared) { g->WG.p[k++] = g->slot[i].wp; --left; }
+    if (k == (size_t)pc::kChainGroupMax || (k && !left)) {
+      unsigned blocks = 0;
+      for (size_t j = 0; j < k; ++j) blocks = std::max(blocks, (unsigned)((g->WG.p[j].n + 255) / 256));
+      g->WG.n = (int)k;
+      g->WG.done_flag = left ? nullptr : flag;
+      g->WG.done_val = want;
+      g->WG.ticket = g->ticket;
+#if defined(PC_EMULATE)
+      pc::emu_chain_wet_group(g->WG);
+#else
+      pc::k_chain_wet_group<<<dim3(blocks, (unsigned)k), 256, 0, g->st>>>(g->WG);
+      if (const cudaError_t e = cudaGetLastError())
+        return group_fail(g, B200CONV_ECUDA, std::string("group wet launch: ") + cudaGetErrorString(e));
+#endif
+      g->launches++;
+      k = 0;
+    }
+  }
+  return 0;
+}
+
+// Commit: head bookkeeping and the tail blocks the launched calls complete, behind the group's event (recorded now if
+// the prepare queued a wait); every prepared member keeps the event for its next own call.  *rc keeps the first error.
+static void group_commit(b200conv_group* g, bool waited, int* rc) {
+  const size_t n = g->m.size();
+  bool recorded = false;
+  if (waited) {
+    if (cudaEventRecord(g->ev, g->st) != cudaSuccess) {
+      cudaGetLastError();
+      if (!*rc) *rc = group_fail(g, B200CONV_ECUDA, "group: event record failed");
+    } else {
+      recorded = true;
+    }
+  }
+  for (size_t i = 0; i < n; ++i) {
+    if (!g->slot[i].launched) continue;
+    if (int crc = rt_commit(g->m[i], g->slot[i].P, g->ev, g->st, &recorded))
+      if (!*rc) *rc = group_member_fail(g, i, crc);
+  }
+  if (recorded)
+    for (size_t i = 0; i < n; ++i)
+      if (g->slot[i].prepared) g->m[i]->grp_ev = g->ev;
+}
+
+// The prepared steps on the group stream: the sends (chain), the convolvers, the wet mixes (chain: the last raises
+// `flag`, the group's word, to `want`, and g->epoch follows it), then the commit.  Nothing is launched once *rc holds
+// an error.
+static void group_launch_round(b200conv_group* g, bool chain, unsigned int* flag, unsigned int want, bool waited,
+                               int* rc) {
+  if (!*rc && chain) *rc = group_chain_sends(g);
+  if (!*rc) *rc = group_launch_classes(g);
+  if (!*rc && chain) {
+    *rc = group_chain_wets(g, flag, want);
+    if (!*rc && flag) g->epoch = want;
+  }
+  group_commit(g, waited, rc);
+}
+
+// wait_word on a word raised by the group stream's work, failing with the group's error
+static int group_wait(b200conv_group* g, const volatile unsigned int* f, unsigned int want) {
+  cudaError_t e = cudaSuccess;
+  if (wait_word(f, want, g->st, &e)) return 0;
+  if (!e) return group_fail(g, B200CONV_ECUDA, "group stream: a completion word was not raised");
+  cudaGetLastError();
+  return group_fail(g, B200CONV_ECUDA, std::string("group stream: ") + cudaGetErrorString(e));
+}
+
+// The members that share a group call's fixed-latency steps, walked in passes as lat_run walks one call; a pass is at
+// most the smallest ring piece among them.  Per pass: every sharing member's input half; then rounds, round q holding
+// the q-th step of every member that completes more than q head blocks in the pass, each prepared as lat_step (or the
+// step of chain_process_latency) runs it, with the member's ring word and sequence value, then launched together and
+// committed on the group stream, so that each member's steps stay in order; then every sharing member's output half.
+// The group stream is ordered behind a member's own steps by main_unsynced, as in a zero-latency group call; a call
+// that launched steps records the group's event once, and the members keep it for their next own call (set_device).
+// chain: in / ysend / yrev are the chain's dry / ysend / yrev tables.  Sets shares_latency for the callers.
+static int group_lat_passes(b200conv_group* g, const float* const* const* in, const float* const* ysend,
+                            const float* const* yrev, float* const* const* out, size_t len, bool chain) {
+  const size_t n = g->m.size();
+  size_t piece = 0;
+  for (size_t i = 0; i < n; ++i) {
+    b200conv* h = g->m[i];
+    GroupSlot& s = g->slot[i];
+    s.nc = group_lat_ctas(g, h, chain);
+    s.shares_latency = s.nc > 0;
+    s.waited = false;
+    if (s.shares_latency) {
+      const LatRing* r = chain ? h->c_lat : h->lat;
+      piece = piece ? std::min(piece, r->piece) : r->piece;
+    }
+  }
+  int rc = 0;
+  bool stepped = false;
+  for (size_t done = 0; done < len && piece && !rc;) {
+    const long long np = (long long)std::min(len - done, piece);
+    long long rounds = 0;
+    for (size_t i = 0; i < n && !rc; ++i) {
+      GroupSlot& s = g->slot[i];
+      if (!s.shares_latency) continue;
+      b200conv* h = g->m[i];
+      LatRing* r = chain ? h->c_lat : h->lat;
+      const float* rows[4] = {};
+      if (chain) { rows[0] = in[i][0]; rows[1] = in[i][1]; rows[2] = ysend ? ysend[i] : nullptr; rows[3] = yrev ? yrev[i] : nullptr; }
+      bool w = false;
+      s.p0 = r->pos;
+      if (int e = lat_in(h, r, chain ? rows : in[i], chain ? 4 : (h->route_on ? h->n_in : h->C), done, np, &w))
+        rc = group_member_fail(g, i, e);
+      if (w) s.waited = true;
+      const long long B = (long long)r->B;
+      rounds = std::max(rounds, (s.p0 + np) / B - s.p0 / B);
+    }
+    for (long long q = 0; q < rounds && !rc; ++q) {
+      bool waited = false;
+      for (size_t i = 0; i < n; ++i) {
+        GroupSlot& s = g->slot[i];
+        s.prepared = s.launched = false;
+        if (!s.shares_latency || rc) continue;
+        b200conv* h = g->m[i];
+        LatRing* r = chain ? h->c_lat : h->lat;
+        const long long k = s.p0 / (long long)r->B + q;
+        if (k >= (s.p0 + np) / (long long)r->B) continue;
+        if ((rc = group_order_behind(g, i, &waited))) continue;
+        const size_t B = r->B, L = r->len, off = (size_t)(k % (long long)r->nslots) * B;
+        const float* d = r->in_dev + off;
+        const unsigned int v = ++r->seq;
+        if ((rc = group_prepare_step(g, i, chain, d, chain ? d + 2 * L : nullptr, chain ? d + 3 * L : nullptr, L,
+                                     r->out_dev + off, L, B, r->word_dev, v, r->ticket, &waited)))
+          continue;
+        r->last_st = g->st;                // lat_wait's fallback synchronises the stream that holds the step
+      }
+      group_launch_round(g, chain, nullptr, 0, waited, &rc);
+      for (size_t i = 0; i < n && !rc; ++i) {
+        const GroupSlot& s = g->slot[i];
+        if (!s.launched) continue;
+        LatRing* r = chain ? g->m[i]->c_lat : g->m[i]->lat;
+        const long long k = s.p0 / (long long)r->B + q;
+        r->slot_seq[k % (long long)r->nslots] = chain ? s.wp.done_val : s.P.done_val;
+        stepped = true;
+      }
+    }
+    for (size_t i = 0; i < n && !rc; ++i) {
+      GroupSlot& s = g->slot[i];
+      if (!s.shares_latency) continue;
+      b200conv* h = g->m[i];
+      bool w = false;
+      if (int e = lat_out(h, chain ? h->c_lat : h->lat, out[i], chain ? 2 : (h->route_on ? h->n_out : h->C), done,
+                          s.p0, np, &w))
+        rc = group_member_fail(g, i, e);
+      if (w) s.waited = true;
+    }
+    done += (size_t)np;
+  }
+  if (stepped) {
+    if (cudaEventRecord(g->ev, g->st) != cudaSuccess) {
+      cudaGetLastError();
+      if (!rc) rc = group_fail(g, B200CONV_ECUDA, "group: event record failed");
+    } else {
+      for (size_t i = 0; i < n; ++i)
+        if (g->slot[i].shares_latency) g->m[i]->grp_ev = g->ev;
+    }
+  }
+  for (size_t i = 0; i < n; ++i)                 // a call that waited counts once in the member's latency_waits
+    if (g->slot[i].waited) g->m[i]->lat_waits++;
+  return rc;
+}
+
+int b200conv_group_process(b200conv_group_t* g, const float* const* const* in, float* const* const* out, size_t len) {
+  if (!g) return B200CONV_EINVAL;
+  if (len == 0) return B200CONV_OK;
+  if (!in || !out) return group_fail(g, B200CONV_EINVAL, "null buffer");
+  const size_t n = g->m.size();
+  // every member's arguments before anything is enqueued: a refused call advances no member
+  for (size_t i = 0; i < n; ++i) {
+    const b200conv* h = g->m[i];
+    if (h->sticky_cuda_error) return group_member_fail(g, i, B200CONV_ECUDA);
+    if (!in[i] || !out[i]) return group_fail(g, B200CONV_EINVAL, "null buffer of member " + std::to_string(i));
+    if (h->lat_D)
+      for (int c = 0; c < (h->route_on ? h->n_in : h->C); ++c)
+        if (!in[i][c]) return group_fail(g, B200CONV_EINVAL, "null buffer of member " + std::to_string(i));
+  }
+  if (cudaSetDevice(g->device) != cudaSuccess) {
+    cudaGetLastError();
+    return group_fail(g, B200CONV_ECUDA, "cudaSetDevice failed");
+  }
+  // the members at the group's fixed latency first, in shared steps
+  int rc = group_lat_passes(g, in, nullptr, nullptr, out, len, false);
+  bool waited = false;
+  // prepare: inputs into the pinned staging, the waits each call needs, its parameters
+  for (size_t i = 0; i < n; ++i) {
+    b200conv* h = g->m[i];
+    GroupSlot& s = g->slot[i];
+    s.prepared = s.launched = false;
+    s.nc = group_ctas(h, len);
+    if (!s.nc || rc) continue;
+    if ((rc = group_order_behind(g, i, &waited))) continue;
+    const int Cin = h->route_on ? h->n_in : h->C;
+    for (int c = 0; c < Cin; ++c) std::memcpy(h->hpin_in + (size_t)c * len, in[i][c], len * sizeof(float));
+    if ((rc = group_prepare_step(g, i, false, h->hpin_in_dev, nullptr, nullptr, len, h->hpin_out_dev, len, len,
+                                 h->hflag_dev, h->flag_epoch + 1, nullptr, &waited)))
+      continue;
+    ++h->flag_epoch;
+  }
+  group_launch_round(g, false, nullptr, 0, waited, &rc);
+  // every other member on its own, while the shared launches run
+  for (size_t i = 0; i < n && !rc; ++i)
+    if (!g->slot[i].nc && !g->slot[i].shares_latency)
+      if (int mrc = b200conv_process(g->m[i], in[i], out[i], len)) rc = group_member_fail(g, i, mrc);
+  // each launched member's completion word, then its output
+  for (size_t i = 0; i < n; ++i) {
+    if (!g->slot[i].launched) continue;
+    const b200conv* h = g->m[i];
+    if (int wrc = group_wait(g, h->hflag, g->slot[i].P.done_val)) return wrc;
+    const int Cout = h->route_on ? h->n_out : h->C;
+    for (int c = 0; c < Cout; ++c) std::memcpy(out[i][c], h->hpin_out + (size_t)c * len, len * sizeof(float));
+  }
+  return rc;
+}
+
+int b200conv_chain_group_process(b200conv_group_t* g, const float* const* const* dry, const float* const* ysend,
+                                 const float* const* yrev, float* const* const* out, size_t len) {
+  if (!g) return B200CONV_EINVAL;
+  if (len == 0) return B200CONV_OK;
+  if (!dry || !out) return group_fail(g, B200CONV_EINVAL, "null buffer");
+  const size_t n = g->m.size();
+  // every member's arguments before anything is enqueued: a refused call advances no member
+  for (size_t i = 0; i < n; ++i) {
+    const b200conv* h = g->m[i];
+    if (h->sticky_cuda_error) return group_member_fail(g, i, B200CONV_ECUDA);
+    if (!h->chain_on) return group_fail(g, B200CONV_ESTATE, "member " + std::to_string(i) + " owns no send / wet chain");
+    if (h->stages.empty() || (h->lat_D && !h->c_lat))
+      return group_fail(g, B200CONV_ESTATE, "member " + std::to_string(i) + " has no impulse response or chain rings");
+    if (!dry[i] || !out[i] || !dry[i][0] || !dry[i][1] || !out[i][0] || !out[i][1])
+      return group_fail(g, B200CONV_EINVAL, "null buffer of member " + std::to_string(i));
+  }
+  if (cudaSetDevice(g->device) != cudaSuccess) {
+    cudaGetLastError();
+    return group_fail(g, B200CONV_ECUDA, "cudaSetDevice failed");
+  }
+  int rc = group_lat_passes(g, dry, ysend, yrev, out, len, true);
+  bool waited = false;
+  size_t shared = 0;
+  // prepare: inputs into the chain's pinned staging, the send / wet parameters, the waits the convolver call needs
+  // and its parameters
+  for (size_t i = 0; i < n; ++i) {
+    b200conv* h = g->m[i];
+    GroupSlot& s = g->slot[i];
+    s.prepared = s.launched = false;
+    s.nc = chain_group_ctas(h, len);
+    if (!s.nc || rc) continue;
+    if ((rc = group_order_behind(g, i, &waited))) continue;
+    const size_t cap = h->hpin_cap;
+    std::memcpy(h->c_hpin, dry[i][0], len * sizeof(float));
+    std::memcpy(h->c_hpin + cap, dry[i][1], len * sizeof(float));
+    const float* ys = ysend ? ysend[i] : nullptr;
+    const float* yr = yrev ? yrev[i] : nullptr;
+    if (ys) std::memcpy(h->c_hpin + 2 * cap, ys, len * sizeof(float));
+    if (yr) std::memcpy(h->c_hpin + 3 * cap, yr, len * sizeof(float));
+    float* d = h->c_hpin_dev;
+    if ((rc = group_prepare_step(g, i, true, d, ys ? d + 2 * cap : nullptr, yr ? d + 3 * cap : nullptr, cap,
+                                 d + 4 * cap, cap, len, nullptr, 0, nullptr, &waited)))
+      continue;
+    ++shared;
+  }
+  // the last wet launch raises the group's word for every shared member
+  const unsigned int want = g->epoch + 1;
+  group_launch_round(g, true, shared ? g->flag_dev : nullptr, want, waited, &rc);
+  // every other member on its own, while the shared launches run
+  for (size_t i = 0; i < n && !rc; ++i)
+    if (!g->slot[i].nc && !g->slot[i].shares_latency)
+      if (int mrc = b200conv_chain_process(g->m[i], dry[i], ysend ? ysend[i] : nullptr, yrev ? yrev[i] : nullptr, out[i],
+                                           len))
+        rc = group_member_fail(g, i, mrc);
+  if (!shared || g->epoch != want) return rc;
+  if (int wrc = group_wait(g, g->flag, want)) return wrc;
+  for (size_t i = 0; i < n; ++i) {
+    if (!g->slot[i].launched) continue;
+    const b200conv* h = g->m[i];
+    for (int ch = 0; ch < 2; ++ch) std::memcpy(out[i][ch], h->c_hpin + (4 + ch) * h->hpin_cap, len * sizeof(float));
+  }
+  return rc;
+}
+
+// A completed b200conv_chain_swap moves the chain to the incoming handle: the caller puts it in the outgoing one's
+// place.  The outgoing handle's next own call must still follow the group's event if it holds it.
+int b200conv_group_set_member(b200conv_group_t* g, int index, b200conv_t* h) {
+  if (!g) return B200CONV_EINVAL;
+  if (index < 0 || (size_t)index >= g->m.size()) return group_fail(g, B200CONV_EINVAL, "member index out of range");
+  if (!h) return group_fail(g, B200CONV_EINVAL, "null member");
+  if (h->cfg.device != g->device) return group_fail(g, B200CONV_EINVAL, "the member is on another device");
+  for (size_t j = 0; j < g->m.size(); ++j)
+    if (g->m[j] == h && (int)j != index) return group_fail(g, B200CONV_EINVAL, "the handle is already a member");
+  b200conv* old = g->m[index];
+  if (old != h && old->grp_ev == g->ev) {
+    cudaError_t e = cudaSetDevice(g->device);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(old->s_main, g->ev, 0);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(old->s_post, g->ev, 0);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      return group_fail(g, B200CONV_ECUDA, std::string("set_member: ") + cudaGetErrorString(e));
+    }
+    old->grp_ev = nullptr;
+  }
+  g->m[index] = h;
+  return B200CONV_OK;
+}
+
+// Every member is checked against b200conv_set_latency's rules before any changes; then each is switched (and cleared)
+// in member order.  samples == 0 switches back only the members in fixed-latency mode.
+int b200conv_group_set_latency(b200conv_group_t* g, size_t samples) {
+  if (!g) return B200CONV_EINVAL;
+  const size_t n = g->m.size();
+  for (size_t i = 0; i < n; ++i) {
+    const b200conv* h = g->m[i];
+    const std::string who = "member " + std::to_string(i) + ": ";
+    if (h->sticky_cuda_error) return group_member_fail(g, i, B200CONV_ECUDA);
+    if (!samples && !h->lat_D) continue;
+    if (h->stages.empty()) return group_fail(g, B200CONV_ESTATE, who + "no impulse response loaded");
+    if (h->cfg.shard_count > 1) return group_fail(g, B200CONV_ESTATE, who + "fixed-latency mode needs an unsharded handle");
+    if (h->p2p_on || h->p2p_tail) return group_fail(g, B200CONV_ESTATE, who + "the slot exchange is attached");
+    if (h->swap_peer) return group_fail(g, B200CONV_ESTATE, who + "an IR hot swap is pending");
+    const size_t B0 = (size_t)h->stages[0].B;
+    if (samples != 0 && (samples % B0 != 0 || samples > 16 * B0))
+      return group_fail(g, B200CONV_EINVAL, who + "the latency must be a multiple of the head block, at most 16 head blocks");
+  }
+  for (size_t i = 0; i < n; ++i) {
+    if (!samples && !g->m[i]->lat_D) continue;
+    if (int rc = b200conv_set_latency(g->m[i], samples)) return group_member_fail(g, i, rc);
+  }
+  g->lat_D = samples;
+  return B200CONV_OK;
+}
+
+size_t b200conv_group_latency(const b200conv_group_t* g) { return g ? g->lat_D : 0; }
 
 int b200conv_clear(b200conv_t* h) {
   REQUIRE_CUDA(h);
