@@ -201,6 +201,40 @@ int                b200conv_group_set_member(b200conv_group_t* g, int index, b20
  * and one wet launch per 32 members, and records one event.  The group call allocates nothing. */
 int                b200conv_group_set_latency(b200conv_group_t* g, size_t samples);
 size_t             b200conv_group_latency(const b200conv_group_t* g);
+/* Group calls on device buffers.  b200conv_group_process_device(g, in_dev, in_stride, out_dev, out_stride, len, sync)
+ * gives member i exactly what b200conv_process_device(members[i], in_dev[i], in_stride[i], out_dev[i], out_stride[i],
+ * len, 0) would; b200conv_chain_group_process_device what b200conv_chain_process_device(members[i], dry_dev[i],
+ * dry_stride[i], ysend_dev ? ysend_dev[i] : NULL, yrev_dev ? yrev_dev[i] : NULL, out_dev[i], out_stride[i], len, 0)
+ * would (ysend_dev / yrev_dev and their entries may be NULL: envelope 1).  Outputs, stage states, filter states and
+ * predelay rings are those calls', in member order, within float rounding; in-place and aliasing rules are theirs.
+ * A member SHARES the group's launches when a one-launch call of it would qualify for b200conv_group_process (length
+ * and staging aside) and its head stage fits one cluster, its call touches at most 16 head blocks counting from its
+ * current fill, and every later stage's block is a multiple of the head block, completes at most once in the call and
+ * its completed block's output is first needed after the call (REEV-R's head 64..1024 / tail 8192 shapes: calls up to
+ * min(16 head blocks, 8192) samples).  A chain member also needs what b200conv_chain_group_process asks, no pending
+ * hot swap, and len < 16384.  Sharing members cost one cluster launch per shape class and 32 members for the whole
+ * call, which walks each member's head blocks inside its cluster (chain: one send launch per send width before, one
+ * wet launch per 32 members after).  Every other member runs its own device call inside the group call.
+ * Stream contract, on the group's stream b200conv_group_stream(g):
+ *  - work the caller enqueued on it before the call happens before the call reads any member's input;
+ *  - work enqueued on it after the call returns sees every member's output;
+ *  - members that run their own call are ordered both ways with it (one event at the start, one per such member at
+ *    the end); sharing members need no event;
+ *  - sync != 0 returns only after the call has completed; the call never spins on a completion word and allocates
+ *    nothing; each member's next own call is ordered behind it.
+ * Errors, checked for every member before anything is enqueued (no member advances): B200CONV_EINVAL for a NULL
+ * table, or a NULL entry with len > 0; B200CONV_ESTATE when the group has a non-zero latency, a member is in
+ * fixed-latency mode, or (chain) a member has no chain or no impulse response; B200CONV_ECUDA for a member whose CUDA
+ * context failed.  len == 0 does nothing.  b200conv_group_launch_count counts the shared launches. */
+int                b200conv_group_process_device(b200conv_group_t* g, const float* const* in_dev,
+                                                 const size_t* in_stride, float* const* out_dev,
+                                                 const size_t* out_stride, size_t len, int sync);
+int                b200conv_chain_group_process_device(b200conv_group_t* g, const float* const* dry_dev,
+                                                       const size_t* dry_stride, const float* const* ysend_dev,
+                                                       const float* const* yrev_dev, float* const* out_dev,
+                                                       const size_t* out_stride, size_t len, int sync);
+/* the cudaStream_t of the group's calls */
+void*              b200conv_group_stream(const b200conv_group_t* g);
 
 /* Introspection --------------------------------------------------------------------------- */
 typedef struct b200conv_stage_info {

@@ -92,6 +92,11 @@ SYMBOLS = [
     ("b200conv_group_set_member", C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     ("b200conv_group_set_latency", C.c_int, [C.c_void_p, C.c_size_t]),
     ("b200conv_group_latency", C.c_size_t, [C.c_void_p]),
+    ("b200conv_group_process_device", C.c_int, [C.c_void_p, _PP, C.POINTER(C.c_size_t), _PP, C.POINTER(C.c_size_t),
+                                                 C.c_size_t, C.c_int]),
+    ("b200conv_chain_group_process_device", C.c_int, [C.c_void_p, _PP, C.POINTER(C.c_size_t), _PP, _PP, _PP,
+                                                       C.POINTER(C.c_size_t), C.c_size_t, C.c_int]),
+    ("b200conv_group_stream", C.c_void_p, [C.c_void_p]),
     ("b200conv_num_stages", C.c_int, [C.c_void_p]),
     ("b200conv_stage", C.c_int, [C.c_void_p, C.c_int, C.POINTER(StageInfo)]),
     ("b200conv_ir_len", C.c_size_t, [C.c_void_p, C.c_int]),

@@ -460,6 +460,41 @@ class Group:
                 C.cast(outs, C.POINTER(C.c_void_p)), n))
         return [(y[0], y[1]) for y in ys]
 
+    def process_device(self, in_ptrs, in_strides, out_ptrs, out_strides, n: int, sync: bool = False) -> None:
+        """engines[i].process_device(in_ptrs[i], in_strides[i], out_ptrs[i], out_strides[i], n) for every i, on the
+        group's stream (b200conv_group_process_device): device addresses (ints), strides in samples.  The members that
+        fit share one cluster launch per shape class for calls of up to 16 head blocks.  Order other streams with
+        `stream`; sync=True returns once the call has completed."""
+        m = len(self.engines)
+        if any(len(t) != m for t in (in_ptrs, in_strides, out_ptrs, out_strides)):
+            raise ValueError("need one buffer and stride per engine")
+        pp = lambda t: (C.c_void_p * m)(*[int(a) for a in t])
+        ss = lambda t: (C.c_size_t * m)(*[int(a) for a in t])
+        self._check(self._l.b200conv_group_process_device(
+            self._g, C.cast(pp(in_ptrs), C.POINTER(C.c_void_p)), ss(in_strides),
+            C.cast(pp(out_ptrs), C.POINTER(C.c_void_p)), ss(out_strides), n, int(sync)))
+
+    def chain_process_device(self, dry_ptrs, dry_strides, out_ptrs, out_strides, n: int, ysend_ptrs=None,
+                             yrev_ptrs=None, sync: bool = False) -> None:
+        """engines[i].chain_process_device(...) for every i on the group's stream (b200conv_chain_group_process_device):
+        dry_ptrs[i] / out_ptrs[i] address L with R one stride later; ysend_ptrs / yrev_ptrs: per-engine envelope
+        addresses (an entry 0 / None, or the whole list None: envelope 1)."""
+        m = len(self.engines)
+        if any(len(t) != m for t in (dry_ptrs, dry_strides, out_ptrs, out_strides)):
+            raise ValueError("need one buffer and stride per engine")
+        if any(t is not None and len(t) != m for t in (ysend_ptrs, yrev_ptrs)):
+            raise ValueError("need one envelope (or None) per engine")
+        pp = lambda t: None if t is None else C.cast((C.c_void_p * m)(*[int(a or 0) for a in t]), C.POINTER(C.c_void_p))
+        ss = lambda t: (C.c_size_t * m)(*[int(a) for a in t])
+        self._check(self._l.b200conv_chain_group_process_device(
+            self._g, pp(dry_ptrs), ss(dry_strides), pp(ysend_ptrs), pp(yrev_ptrs), pp(out_ptrs), ss(out_strides), n,
+            int(sync)))
+
+    @property
+    def stream(self) -> int:
+        """the cudaStream_t of the group's calls, e.g. for torch.cuda.ExternalStream"""
+        return int(self._l.b200conv_group_stream(self._g) or 0)
+
     def set_member(self, i: int, engine: Engine) -> None:
         """engines[i] = engine (b200conv_group_set_member), e.g. the incoming engine of a completed chain_swap"""
         self._check(self._l.b200conv_group_set_member(self._g, i, engine._h))

@@ -280,6 +280,9 @@ struct b200conv {
   // orders s_main and s_post behind (nullptr: none)
   bool main_unsynced = false;
   cudaEvent_t grp_ev = nullptr;
+  // a device-buffer group call leaves no event behind: grp_ev is recorded on grp_st (the group's stream) by this
+  // handle's next own call, in set_device (nullptr: nothing to record)
+  cudaStream_t grp_st = nullptr;
 };
 
 namespace {
@@ -1124,6 +1127,10 @@ int launch_cmac_exchange(b200conv* h, const pc::CmacParams& P, int C, const Tail
 int set_device(b200conv* h) {
   CU_CHECK(h, cudaSetDevice(h->cfg.device));
   h->main_unsynced = true;
+  if (h->grp_st) {
+    CU_CHECK(h, cudaEventRecord(h->grp_ev, h->grp_st));
+    h->grp_st = nullptr;
+  }
   if (h->grp_ev) {
     CU_CHECK(h, cudaStreamWaitEvent(h->s_main, h->grp_ev, 0));
     CU_CHECK(h, cudaStreamWaitEvent(h->s_post, h->grp_ev, 0));
@@ -2144,7 +2151,11 @@ template <int M>
 cudaError_t rt_launch_m(const pc::RtGroupParams& G, int cluster, size_t smem, cudaStream_t st) {
   return rt_launch_kernel(pc::k_rt_group<M>, G, G.n * cluster, cluster, smem, st);
 }
-// k_rt_block<M> (one call) or k_rt_group<M> (a group's shape class) with clusters of C * NC CTAs
+template <int M>
+cudaError_t rt_launch_m(const pc::RtStepGroupParams& G, int cluster, size_t smem, cudaStream_t st) {
+  return rt_launch_kernel(pc::k_rt_group_steps<M>, G, G.n * cluster, cluster, smem, st);
+}
+// k_rt_block<M> (one call), k_rt_group<M> or k_rt_group_steps<M> (a group's shape class) with clusters of C * NC CTAs
 template <class Arg>
 cudaError_t rt_launch(const Arg& a, int M, int C, int NC, cudaStream_t st) {
   const size_t smem = (size_t)pc::rt_smem_layout(M, C).bytes;
@@ -2165,7 +2176,9 @@ bool rt_set_attr() {
   return cudaFuncSetAttribute(pc::k_rt_block<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
          cudaFuncSetAttribute(pc::k_rt_block<M>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess &&
          cudaFuncSetAttribute(pc::k_rt_group<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
-         cudaFuncSetAttribute(pc::k_rt_group<M>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
+         cudaFuncSetAttribute(pc::k_rt_group<M>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess &&
+         cudaFuncSetAttribute(pc::k_rt_group_steps<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
+         cudaFuncSetAttribute(pc::k_rt_group_steps<M>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
 }
 #endif
 
@@ -2173,8 +2186,10 @@ bool rt_set_attr() {
 // handles, launches them together and commits them.  `in` / `out` are device-accessible (pinned host or device memory).
 // Prepare: the waits for tail outputs the call needs and room in the timeline, both queued on `st`, the stream the launch
 // goes to (*waited is set if there was a wait), and the call's parameters.  Split mode (nc < 0) is set up by rt_call.
+// With T (the step form of the device-buffer group calls, group_step_ctas() > 0), P is T->p and the call of up to
+// kRtMaxSteps head blocks becomes one step record: the kernel derives its segments from the call's start.
 int rt_prepare(b200conv* h, int nc, const float* in, size_t in_stride, float* out, size_t out_stride, size_t len,
-               cudaStream_t st, pc::RtParams& P, bool* waited) {
+               cudaStream_t st, pc::RtParams& P, bool* waited, pc::RtStepParams* T = nullptr) {
   const int C = h->C;
   Stage& s0 = h->stages[0];
   const int M = s0.B;
@@ -2191,10 +2206,12 @@ int rt_prepare(b200conv* h, int nc, const float* in, size_t in_stride, float* ou
   }
   // a call that crosses the block boundary: len1 samples complete the open block, the other r start the next one
   const int len1 = std::min((int)len, M - s0.fill), r = (int)len - len1;
-  if (int rc = ensure_rows(h, s0, r ? 2 : 1, st)) return rc;
+  const int nrows = T ? 1 + (r + M - 1) / M : (r ? 2 : 1);
+  if (int rc = ensure_rows(h, s0, nrows, st)) return rc;
+  if (T) *T = pc::RtStepParams{};
   P = pc::RtParams{};
   P.M = M; P.C = C; P.NC = nc; P.P = s0.P;
-  P.len = (int)len; P.nseg = r ? 2 : 1;
+  P.len = (int)len; P.nseg = T ? 0 : (r ? 2 : 1);
   pc::RtSeg& S1 = P.seg[0];
   pc::RtSeg& S2 = P.seg[1];
   S1.fill = s0.fill; S1.len = len1; S1.complete = (s0.fill + len1 == M) ? 1 : 0; S1.off = 0;
@@ -2206,16 +2223,23 @@ int rt_prepare(b200conv* h, int nc, const float* in, size_t in_stride, float* ou
   P.inbuf0 = s0.inbuf; P.inbuf0_stride = (long long)s0.in_stride;
   P.H = s0.H; P.h_cstride = (long long)s0.Prows * M;
   P.X = s0.X; P.x_cstride = (long long)s0.R * M;
-  P.Yprev = s0.Y[s0.ybuf]; P.Ynext = s0.Y[s0.ybuf ^ 1]; P.y_cstride = M;
+  // the step form stores only the last completed block's spectrum, where the one-launch calls would have left it
+  const int ncomplete = (s0.fill + (int)len) / M;
+  P.Yprev = s0.Y[s0.ybuf]; P.Ynext = s0.Y[T ? s0.ybuf ^ (ncomplete & 1) : s0.ybuf ^ 1]; P.y_cstride = M;
   P.tw = s0.tw;
   int na = 0;
   for (size_t si = 1; si < h->stages.size(); ++si) {
     Stage& s = h->stages[si];
     P.later_stride[na] = (long long)s.in_stride;
     S1.later_inbuf[na] = s.inbuf; S1.later_fill[na] = s.fill;
-    // a stage whose block completes at the boundary takes the samples after it at the front of its other buffer
-    const bool at_boundary = r && s.fill + len1 == s.B;
+    // a stage whose block completes at the boundary takes the samples after it at the front of its other buffer (the
+    // step form: at the one boundary group_step_ctas allows inside the call)
+    const bool at_boundary = T ? s.fill + (int)len > s.B : (r && s.fill + len1 == s.B);
     S2.later_inbuf[na] = at_boundary ? s.inbuf_alt : s.inbuf; S2.later_fill[na] = at_boundary ? 0 : s.fill + len1;
+    if (T) {
+      T->later_inbuf[na] = s.inbuf; T->later_alt[na] = s.inbuf_alt;
+      T->later_fill[na] = s.fill; T->later_B[na] = s.B;
+    }
     // That buffer was read by the stage's previous tail block on s_tail, so s_main must be ordered behind it.  With
     // q <= 2 (every two-stage handle) the loop above has already waited for it, as it does for the first call after the
     // buffer swap below: that block's output starts at (blocks_done - 1 + q) * B, at or before the boundary, and this
@@ -2234,23 +2258,29 @@ int rt_prepare(b200conv* h, int nc, const float* in, size_t in_stride, float* ou
   P.out = out; P.out_stride = (long long)out_stride;
   P.mix_on = h->route_on ? 1 : 0; P.n_out = h->route_on ? h->n_out : C;
   std::memcpy(P.mix, h->mix, sizeof(P.mix));
+  if (T) {
+    P.seg[0] = P.seg[1] = pc::RtSeg{};
+    T->fill = s0.fill; T->head = s0.head; T->abs_pos = h->abs_pos;
+  }
   return 0;
 }
 
-// Commit: the bookkeeping of a launched call and the tail blocks it completes.  They go to the low-priority stream
-// behind event `ev`, which is recorded on `st` (behind the call's launch) by the first of them unless *recorded.
-int rt_commit(b200conv* h, const pc::RtParams& P, cudaEvent_t ev, cudaStream_t st, bool* recorded) {
+// Commit: the bookkeeping of a launched call of len samples, as the one-launch calls of its head-block pieces would
+// leave it, and the tail blocks it completes (at most one per stage).  They go to the low-priority stream behind event
+// `ev`, which is recorded on `st` (behind the call's launch) by the first of them unless *recorded.
+int rt_commit(b200conv* h, int len, cudaEvent_t ev, cudaStream_t st, bool* recorded) {
   Stage& s0 = h->stages[0];
-  const int len1 = P.seg[0].len, r = P.len - len1;
-  // bookkeeping of the head stage
-  if (P.seg[0].complete) { s0.head += 1; s0.blocks_done += 1; s0.fill = r; s0.ybuf ^= 1; }
-  else s0.fill += P.len;
-  h->abs_pos += (long long)P.len;
+  // bookkeeping of the head stage: every completed block advances the timeline and flips the overlap buffer
+  const int ncomplete = (s0.fill + len) / s0.B;
+  s0.head += ncomplete; s0.blocks_done += ncomplete; s0.ybuf ^= ncomplete & 1;
+  s0.fill = (s0.fill + len) % s0.B;
+  h->abs_pos += (long long)len;
   // later stages: the kernel appended the samples; a completed block goes to the low-priority stream
   for (size_t si = 1; si < h->stages.size(); ++si) {
     Stage& s = h->stages[si];
-    s.fill += len1;
-    if (s.fill < s.B) { s.fill += r; continue; }
+    s.fill += len;
+    if (s.fill < s.B) continue;
+    const int rest = s.fill - s.B;
     if (!*recorded) { CU_CHECK(h, cudaEventRecord(ev, st)); *recorded = true; }
     CU_CHECK(h, cudaStreamWaitEvent(h->s_tail, ev, 0));
     const int j = (int)(s.njobs & 1);
@@ -2263,7 +2293,7 @@ int rt_commit(b200conv* h, const pc::RtParams& P, cudaEvent_t ev, cudaStream_t s
     s.job_waited[j] = false;
     s.njobs++;
     std::swap(s.inbuf, s.inbuf_alt);              // the following calls fill the other buffer
-    s.fill = r;                                   // ... which holds the samples after the boundary
+    s.fill = rest;                                // ... which holds the samples after the boundary
   }
   return 0;
 }
@@ -2304,7 +2334,7 @@ int rt_call(b200conv* h, int nc, const float* in, size_t in_stride, float* out, 
     if (int rc = rt_launch_one(h, P)) return rc;
   }
   bool recorded = false;
-  return rt_commit(h, P, h->ev_rt, h->s_main, &recorded);
+  return rt_commit(h, P.len, h->ev_rt, h->s_main, &recorded);
 }
 
 // Waits until the pinned completion word *f reached `want`: spins, and after 20 ms synchronises st, the stream that
@@ -3791,7 +3821,7 @@ int b200conv_chain_swap_state(const b200conv_t* h) { return h ? h->swap_state : 
 
 // A member's part of the step a group call is running
 struct GroupSlot {
-  pc::RtParams P;                    // the convolver call
+  pc::RtStepParams R;                // the convolver call (R.p), with its step walk in the step form
   pc::ChainSendParams sp;            // a chain member's send and wet mix
   pc::ChainWetParams wp;
   int nc = 0;                        // cluster width of a member that shares the launches, 0: it runs its own call
@@ -3811,6 +3841,7 @@ struct b200conv_group {
   // per-call scratch, sized by create: a group call allocates nothing
   std::vector<GroupSlot> slot;
   pc::RtGroupParams G;                   // the tables of one launch
+  pc::RtStepGroupParams GS;
   pc::ChainSendGroupParams SG;
   pc::ChainWetGroupParams WG;
   // b200conv_chain_group_process: the group's pinned completion word (+ its device-side address) and the wet launch's
@@ -3857,6 +3888,32 @@ static int group_lat_ctas(const b200conv_group* g, const b200conv* h, bool chain
   return std::max(rt_cluster_ctas(h, h->stages[0].B), 0);
 }
 
+// Device-buffer group calls (b200conv_group_process_device, b200conv_chain_group_process_device): a member shares the
+// group's k_rt_group_steps launches when a one-launch call of it would (group_ctas without the length and host-staging
+// rules, not in split mode), its call touches at most kRtMaxSteps head blocks from its fill on, and every later stage
+// has a block that is a multiple of the head block, completes at most once in the call, and whose completed block's
+// output is first needed after the call (the crossing rule of rt_cluster_ctas for any number of head blocks).  A chain
+// member also meets chain_group_ctas' rules and len stays below kChainWideMin, where b200conv_chain_process_device
+// runs the serial send.  Its cluster width, else 0.
+static int group_step_ctas(const b200conv* h, size_t len, bool chain) {
+  if (h->cfg.shard_count != 1 || h->lat_D || h->stages.empty() || len == 0) return 0;
+  if (chain && (!h->chain.on || h->swap_peer || !h->opt_rt || len > h->Lmax - h->stages[0].B || len >= kChainWideMin))
+    return 0;
+  const Stage& s0 = h->stages[0];
+  const long long M = s0.B, n = (long long)len;
+  const long long len1 = std::min(n, M - s0.fill);
+  if (1 + (n - len1 + M - 1) / M > pc::kRtMaxSteps) return 0;
+  for (size_t si = 1; si < h->stages.size(); ++si) {
+    const Stage& s = h->stages[si];
+    const long long d = s.B - s.fill;                 // samples of the call up to the stage's block boundary
+    if (s.B % M != 0) return 0;
+    if (d <= n && (d < len1 || (d - len1) % M != 0 || n - d >= s.B ||
+                   h->abs_pos + n > (s.blocks_done + s.q) * (long long)s.B))
+      return 0;
+  }
+  return std::max(rt_cluster_ctas(h, 1), 0);        // the width of a call inside the open block; -1 (split): 0
+}
+
 b200conv_group_t* b200conv_group_create(b200conv_t* const* members, int n) {
   if (!members || n < 1 || n > 64) return nullptr;
   for (int i = 0; i < n; ++i) {
@@ -3900,7 +3957,7 @@ void b200conv_group_destroy(b200conv_group_t* g) {
   cudaSetDevice(g->device);
   if (g->st) cudaStreamSynchronize(g->st);
   for (b200conv* h : g->m) {
-    if (h->grp_ev == g->ev) h->grp_ev = nullptr;        // everything the event covers has completed
+    if (h->grp_ev == g->ev) h->grp_ev = nullptr, h->grp_st = nullptr;   // everything the event covers has completed
     for (LatRing* r : {h->lat, h->chain.lat})          // ... and every step the group stream held
       if (r && r->last_st == g->st) r->last_st = h->s_main;
   }
@@ -3928,7 +3985,8 @@ static int group_order_behind(b200conv_group* g, size_t i, bool* waited) {
 }
 
 // Prepares member i's step of len samples on the group stream (its waits and a timeline compaction go there; *waited is
-// set if there was a wait).  in: the input rows, in_stride apart; for a chain member the dry rows, with the send / rev
+// set if there was a wait); `steps`: the step form of a device-buffer group call (a call of up to kRtMaxSteps head
+// blocks, k_rt_group_steps).  in: the input rows, in_stride apart; for a chain member the dry rows, with the send / rev
 // envelope rows (nullptr: envelope 1).  out: the output rows, out_stride apart.  flag / val: the step's completion word
 // and value, ticket: the wet kernel's ticket word of a chain member (nullptr / 0: none).  A chain member's send and wet
 // are those of chain_piece's k_chain_send form with the row of the handle's configuration, and the chain moves past
@@ -3936,7 +3994,8 @@ static int group_order_behind(b200conv_group* g, size_t i, bool* waited) {
 // prepared even if this fails: waits may have been queued.
 static int group_prepare_step(b200conv_group* g, size_t i, bool chain, const float* in, const float* send,
                               const float* rev, size_t in_stride, float* out, size_t out_stride, size_t len,
-                              unsigned int* flag, unsigned int val, unsigned int* ticket, bool* waited) {
+                              unsigned int* flag, unsigned int val, unsigned int* ticket, bool* waited,
+                              bool steps = false) {
   b200conv* h = g->m[i];
   GroupSlot& s = g->slot[i];
   int rc;
@@ -3946,37 +4005,40 @@ static int group_prepare_step(b200conv_group* g, size_t i, bool chain, const flo
     h->chain.ring_pos += (long long)len;
     s.wp.done_flag = flag; s.wp.done_val = val; s.wp.ticket = ticket;
     h->route_in_only = true;
-    rc = rt_prepare(h, s.nc, h->chain.conv_in, h->Lmax, h->dch[0], h->Lmax, len, g->st, s.P, waited);
+    rc = rt_prepare(h, s.nc, h->chain.conv_in, h->Lmax, h->dch[0], h->Lmax, len, g->st, s.R.p, waited,
+                    steps ? &s.R : nullptr);
     h->route_in_only = false;
   } else {
-    rc = rt_prepare(h, s.nc, in, in_stride, out, out_stride, len, g->st, s.P, waited);
-    s.P.done_flag = flag; s.P.done_val = val;
+    rc = rt_prepare(h, s.nc, in, in_stride, out, out_stride, len, g->st, s.R.p, waited, steps ? &s.R : nullptr);
+    s.R.p.done_flag = flag; s.R.p.done_val = val;
   }
   s.prepared = true;
   return rc ? group_member_fail(g, i, rc) : 0;
 }
 
-// The prepared members' clusters: one k_rt_group launch per shape class (M, C, NC) and kRtGroupMax members, in
-// member order within a class, on the group stream
-static int group_launch_classes(b200conv_group* g) {
+// The prepared members' clusters: one k_rt_group launch (steps: k_rt_group_steps) per shape class (M, C, NC) and
+// kRtGroupMax members, in member order within a class, on the group stream
+static int group_launch_classes(b200conv_group* g, bool steps) {
   const size_t n = g->m.size();
   for (size_t i = 0; i < n; ++i) {
     if (!g->slot[i].prepared || g->slot[i].launched) continue;
-    const pc::RtParams& A = g->slot[i].P;
+    const pc::RtParams& A = g->slot[i].R.p;
     size_t idx[pc::kRtGroupMax];
     int k = 0;
     for (size_t j = i; j < n && k < pc::kRtGroupMax; ++j) {
       const GroupSlot& s = g->slot[j];
-      if (s.prepared && !s.launched && s.P.M == A.M && s.P.C == A.C && s.P.NC == A.NC) {
-        g->G.p[k] = s.P;
+      if (s.prepared && !s.launched && s.R.p.M == A.M && s.R.p.C == A.C && s.R.p.NC == A.NC) {
+        if (steps) g->GS.p[k] = s.R;
+        else g->G.p[k] = s.R.p;
         idx[k++] = j;
       }
     }
-    g->G.n = k;
+    g->G.n = g->GS.n = k;
 #if defined(PC_EMULATE)
-    pc::emu_rt_group(g->G);
+    if (steps) pc::emu_rt_group_steps(g->GS);
+    else pc::emu_rt_group(g->G);
 #else
-    if (const cudaError_t e = rt_launch(g->G, A.M, A.C, A.NC, g->st)) {
+    if (const cudaError_t e = steps ? rt_launch(g->GS, A.M, A.C, A.NC, g->st) : rt_launch(g->G, A.M, A.C, A.NC, g->st)) {
       cudaGetLastError();
       return group_fail(g, B200CONV_ECUDA, std::string("group launch: ") + cudaGetErrorString(e));
     }
@@ -4057,7 +4119,7 @@ static void group_commit(b200conv_group* g, bool waited, int* rc) {
   }
   for (size_t i = 0; i < n; ++i) {
     if (!g->slot[i].launched) continue;
-    if (int crc = rt_commit(g->m[i], g->slot[i].P, g->ev, g->st, &recorded))
+    if (int crc = rt_commit(g->m[i], g->slot[i].R.p.len, g->ev, g->st, &recorded))
       if (!*rc) *rc = group_member_fail(g, i, crc);
   }
   if (recorded)
@@ -4065,13 +4127,13 @@ static void group_commit(b200conv_group* g, bool waited, int* rc) {
       if (g->slot[i].prepared) g->m[i]->grp_ev = g->ev;
 }
 
-// The prepared steps on the group stream: the sends (chain), the convolvers, the wet mixes (chain: the last raises
-// `flag`, the group's word, to `want`, and g->epoch follows it), then the commit.  Nothing is launched once *rc holds
-// an error.
+// The prepared steps on the group stream: the sends (chain), the convolvers (steps: in the step form), the wet mixes
+// (chain: the last raises `flag`, the group's word, to `want`, and g->epoch follows it), then the commit.  Nothing is
+// launched once *rc holds an error.
 static void group_launch_round(b200conv_group* g, bool chain, unsigned int* flag, unsigned int want, bool waited,
-                               int* rc) {
+                               int* rc, bool steps = false) {
   if (!*rc && chain) *rc = group_chain_sends(g);
-  if (!*rc) *rc = group_launch_classes(g);
+  if (!*rc) *rc = group_launch_classes(g, steps);
   if (!*rc && chain) {
     *rc = group_chain_wets(g, flag, want);
     if (!*rc && flag) g->epoch = want;
@@ -4156,7 +4218,7 @@ static int group_lat_passes(b200conv_group* g, const float* const* const* in, co
         if (!s.launched) continue;
         LatRing* r = chain ? g->m[i]->chain.lat : g->m[i]->lat;
         const long long k = s.p0 / (long long)r->B + q;
-        r->slot_seq[k % (long long)r->nslots] = chain ? s.wp.done_val : s.P.done_val;
+        r->slot_seq[k % (long long)r->nslots] = chain ? s.wp.done_val : s.R.p.done_val;
         stepped = true;
       }
     }
@@ -4231,7 +4293,7 @@ int b200conv_group_process(b200conv_group_t* g, const float* const* const* in, f
   for (size_t i = 0; i < n; ++i) {
     if (!g->slot[i].launched) continue;
     const b200conv* h = g->m[i];
-    if (int wrc = group_wait(g, h->hflag, g->slot[i].P.done_val)) return wrc;
+    if (int wrc = group_wait(g, h->hflag, g->slot[i].R.p.done_val)) return wrc;
     const int Cout = h->route_on ? h->n_out : h->C;
     for (int c = 0; c < Cout; ++c) std::memcpy(out[i][c], h->hpin_out + (size_t)c * len, len * sizeof(float));
   }
@@ -4292,6 +4354,125 @@ int b200conv_chain_group_process(b200conv_group_t* g, const float* const* const*
   return rc;
 }
 
+// ---- device-buffer group calls --------------------------------------------------------------------------------------
+// Every launch goes to the group stream and nothing waits on the host.  The members that share (group_step_ctas) run
+// their whole call in the step form: one k_rt_group_steps launch per shape class (chain: the sends before, the wet
+// mixes after), with no completion word; their next own call records the group's event lazily (grp_st, set_device).
+// Every other member runs its own device call on its own streams, ordered both ways with the group stream: behind one
+// event recorded at the start, and the group stream behind each such member's s_main at the end.
+
+// the checks of both entries that need no member's kind: a refused call advances no member
+// (tables: every buffer and stride table is there)
+static int group_device_check(b200conv_group* g, bool chain, bool tables, const float* const* in_dev,
+                              float* const* out_dev, size_t len) {
+  if (!tables) return group_fail(g, B200CONV_EINVAL, "null table");
+  if (len == 0) return B200CONV_OK;
+  if (g->lat_D) return group_fail(g, B200CONV_ESTATE, "device-pointer group calls are not available at a fixed latency");
+  for (size_t i = 0; i < g->m.size(); ++i) {
+    const b200conv* h = g->m[i];
+    const std::string who = "member " + std::to_string(i);
+    if (h->sticky_cuda_error) return group_member_fail(g, i, B200CONV_ECUDA);
+    if (h->lat_D) return group_fail(g, B200CONV_ESTATE, who + " is in fixed-latency mode");
+    if (chain && !h->chain.on) return group_fail(g, B200CONV_ESTATE, who + " owns no send / wet chain");
+    if (chain && h->stages.empty()) return group_fail(g, B200CONV_ESTATE, who + " has no impulse response");
+    if (!in_dev[i] || !out_dev[i]) return group_fail(g, B200CONV_EINVAL, "null buffer of member " + std::to_string(i));
+  }
+  if (cudaSetDevice(g->device) != cudaSuccess) {
+    cudaGetLastError();
+    return group_fail(g, B200CONV_ECUDA, "cudaSetDevice failed");
+  }
+  return B200CONV_OK;
+}
+
+// One device-buffer group call: `own(i)` runs member i's own device call.  The sharing members were chosen and
+// prepared by the caller (slot.nc, slot.prepared); this launches them, runs the others and orders the streams.
+extern "C++" {
+template <class Own>
+static int group_device_run(b200conv_group* g, bool chain, bool waited, int rc, int sync, Own own) {
+  const size_t n = g->m.size();
+  bool any_own = false;
+  for (size_t i = 0; i < n; ++i) any_own |= !g->slot[i].nc;
+  if (!rc && any_own) {
+    cudaError_t e = cudaEventRecord(g->ev, g->st);
+    for (size_t i = 0; i < n && e == cudaSuccess; ++i)
+      if (!g->slot[i].nc) e = cudaStreamWaitEvent(g->m[i]->s_main, g->ev, 0);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      rc = group_fail(g, B200CONV_ECUDA, std::string("group: ordering the members' streams: ") + cudaGetErrorString(e));
+    }
+  }
+  group_launch_round(g, chain, nullptr, 0, waited, &rc, true);
+  for (size_t i = 0; i < n; ++i)
+    if (g->slot[i].prepared) { g->m[i]->grp_ev = g->ev; g->m[i]->grp_st = g->st; }
+  for (size_t i = 0; i < n && !rc; ++i) {
+    if (g->slot[i].nc) continue;
+    b200conv* h = g->m[i];
+    if (int mrc = own(i)) { rc = group_member_fail(g, i, mrc); break; }
+    cudaError_t e = cudaEventRecord(h->ev_rt, h->s_main);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(g->st, h->ev_rt, 0);
+    if (e != cudaSuccess) rc = group_member_fail(g, i, cuda_fail(h, e, "group: ordering the group stream behind the member"));
+  }
+  if (!rc && sync) {
+    if (const cudaError_t e = cudaStreamSynchronize(g->st)) {
+      cudaGetLastError();
+      return group_fail(g, B200CONV_ECUDA, std::string("group stream: ") + cudaGetErrorString(e));
+    }
+  }
+  return rc;
+}
+}  // extern "C++"
+
+int b200conv_group_process_device(b200conv_group_t* g, const float* const* in_dev, const size_t* in_stride,
+                                  float* const* out_dev, const size_t* out_stride, size_t len, int sync) {
+  if (!g) return B200CONV_EINVAL;
+  if (int rc = group_device_check(g, false, in_dev && in_stride && out_dev && out_stride, in_dev, out_dev, len))
+    return rc;
+  if (len == 0) return B200CONV_OK;
+  const size_t n = g->m.size();
+  int rc = 0;
+  bool waited = false;
+  for (size_t i = 0; i < n; ++i) {
+    GroupSlot& s = g->slot[i];
+    s.prepared = s.launched = false;
+    s.nc = group_step_ctas(g->m[i], len, false);
+    if (!s.nc || rc) continue;
+    if ((rc = group_order_behind(g, i, &waited))) continue;
+    rc = group_prepare_step(g, i, false, in_dev[i], nullptr, nullptr, in_stride[i], out_dev[i], out_stride[i], len,
+                            nullptr, 0, nullptr, &waited, true);
+  }
+  return group_device_run(g, false, waited, rc, sync, [&](size_t i) {
+    return b200conv_process_device(g->m[i], in_dev[i], in_stride[i], out_dev[i], out_stride[i], len, 0);
+  });
+}
+
+int b200conv_chain_group_process_device(b200conv_group_t* g, const float* const* dry_dev, const size_t* dry_stride,
+                                        const float* const* ysend_dev, const float* const* yrev_dev,
+                                        float* const* out_dev, const size_t* out_stride, size_t len, int sync) {
+  if (!g) return B200CONV_EINVAL;
+  if (int rc = group_device_check(g, true, dry_dev && dry_stride && out_dev && out_stride, dry_dev, out_dev, len))
+    return rc;
+  if (len == 0) return B200CONV_OK;
+  const size_t n = g->m.size();
+  int rc = 0;
+  bool waited = false;
+  for (size_t i = 0; i < n; ++i) {
+    GroupSlot& s = g->slot[i];
+    s.prepared = s.launched = false;
+    s.nc = group_step_ctas(g->m[i], len, true);
+    if (!s.nc || rc) continue;
+    if ((rc = group_order_behind(g, i, &waited))) continue;
+    rc = group_prepare_step(g, i, true, dry_dev[i], ysend_dev ? ysend_dev[i] : nullptr,
+                            yrev_dev ? yrev_dev[i] : nullptr, dry_stride[i], out_dev[i], out_stride[i], len, nullptr, 0,
+                            nullptr, &waited, true);
+  }
+  return group_device_run(g, true, waited, rc, sync, [&](size_t i) {
+    return b200conv_chain_process_device(g->m[i], dry_dev[i], dry_stride[i], ysend_dev ? ysend_dev[i] : nullptr,
+                                         yrev_dev ? yrev_dev[i] : nullptr, out_dev[i], out_stride[i], len, 0);
+  });
+}
+
+void* b200conv_group_stream(const b200conv_group_t* g) { return g ? (void*)g->st : nullptr; }
+
 // A completed b200conv_chain_swap moves the chain to the incoming handle: the caller puts it in the outgoing one's
 // place.  The outgoing handle's next own call must still follow the group's event if it holds it.
 int b200conv_group_set_member(b200conv_group_t* g, int index, b200conv_t* h) {
@@ -4304,6 +4485,7 @@ int b200conv_group_set_member(b200conv_group_t* g, int index, b200conv_t* h) {
   b200conv* old = g->m[index];
   if (old != h && old->grp_ev == g->ev) {
     cudaError_t e = cudaSetDevice(g->device);
+    if (e == cudaSuccess && old->grp_st) e = cudaEventRecord(g->ev, g->st);
     if (e == cudaSuccess) e = cudaStreamWaitEvent(old->s_main, g->ev, 0);
     if (e == cudaSuccess) e = cudaStreamWaitEvent(old->s_post, g->ev, 0);
     if (e != cudaSuccess) {
@@ -4311,6 +4493,7 @@ int b200conv_group_set_member(b200conv_group_t* g, int index, b200conv_t* h) {
       return group_fail(g, B200CONV_ECUDA, std::string("set_member: ") + cudaGetErrorString(e));
     }
     old->grp_ev = nullptr;
+    old->grp_st = nullptr;
   }
   g->m[index] = h;
   return B200CONV_OK;

@@ -27,6 +27,9 @@
 // segment and its overlap spectrum from the q = 0 CTA's yfull of the first segment, so nothing the launch writes to
 // global memory is read back inside it; the cluster barrier of phase D separates the segments.
 //
+// k_rt_group_steps generalises the crossing call to a walk of up to kRtMaxSteps head blocks (device-buffer group
+// calls, RtStepParams).
+//
 // The host keeps the bookkeeping (fill, head, buffer parity); tail stages whose block completes in the call are
 // enqueued on a low-priority stream and consumed one tail period later (TwoStageFFTConvolver.cpp:213-222).
 #pragma once
@@ -83,6 +86,53 @@ struct RtGroupParams {
   RtParams p[kRtGroupMax];
 };
 static_assert(sizeof(RtGroupParams) <= 32764, "k_rt_group's parameter table exceeds the kernel-parameter limit");
+
+// The step form (k_rt_group_steps, the device-buffer group calls): one member's call of up to kRtMaxSteps head blocks,
+// walked in one cluster as consecutive segments (the rest of the open block, whole head blocks, a final partial
+// block), each running phases A-E as the reference runs its FFTConvolver::process loop.  `p` carries everything but
+// the segments (p.nseg = 0); the kernel derives them from the call's start (rt_step_seg), so the record stays the same
+// size for any call length.
+constexpr int kRtMaxSteps = 16;
+struct RtStepParams {
+  RtParams p;
+  int fill;                  // samples of the open head block before the call
+  long long head;            // its timeline row
+  long long abs_pos;         // stream position of the call's first sample
+  // later stage s: open block later_inbuf[s] holds later_fill[s] of its later_B[s] samples; the samples after the one
+  // boundary where its block completes go to the front of later_alt[s]
+  float* later_inbuf[3]; float* later_alt[3]; int later_fill[3]; int later_B[3];
+};
+struct RtStepGroupParams {
+  int n;
+  RtStepParams p[kRtGroupMax];
+};
+static_assert(sizeof(RtStepGroupParams) <= 32764, "k_rt_group_steps' parameter table exceeds the kernel-parameter limit");
+
+// segments of a step-form call
+PC_HD int rt_step_count(const RtStepParams& T) {
+  const int M = T.p.M, len1 = T.p.len < M - T.fill ? T.p.len : M - T.fill;
+  return 1 + (T.p.len - len1 + M - 1) / M;
+}
+// Segment g of a step-form call.  `complete` marks only the LAST block the call completes: that step alone stores
+// the overlap spectrum Ynext, which the host picked with the parity the equivalent one-launch calls would leave (with
+// an even number of completed blocks it is Yprev, read by step 0 before any later step stores).
+PC_HD RtSeg rt_step_seg(const RtStepParams& T, int g) {
+  const int M = T.p.M, len1 = T.p.len < M - T.fill ? T.p.len : M - T.fill;
+  RtSeg S;
+  S.fill = g ? 0 : T.fill;
+  S.off = g ? len1 + (g - 1) * M : 0;
+  S.len = T.p.len - S.off < M - S.fill ? T.p.len - S.off : M - S.fill;
+  S.complete = (g == (T.fill + T.p.len) / M - 1) ? 1 : 0;
+  S.head = T.head + g;
+  S.abs0 = T.abs_pos + S.off - S.fill;
+  for (int s = 0; s < T.p.n_later; ++s) {
+    const int f = T.later_fill[s] + S.off;
+    const bool alt = f >= T.later_B[s];
+    S.later_inbuf[s] = alt ? T.later_alt[s] : T.later_inbuf[s];
+    S.later_fill[s] = alt ? f - T.later_B[s] : f;
+  }
+  return S;
+}
 
 // shared-memory layout of one CTA (float2 units unless noted); xnew and yfull hold one row per segment, MB apart
 struct RtSmem {
@@ -150,8 +200,22 @@ PC_HD void rt_assemble(const RtParams& P, const RtSeg& S, int c, int q, int i, f
   xs[i] = v;
 }
 
+// a timeline pair the same launch may have stored (step form): a coherent load, never the read-only path
+PC_HD float4c ld_pair_live(const float2* p) {
+#if defined(__CUDA_ARCH__)
+  float4 v;
+  asm volatile("ld.global.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p) : "memory");
+  float4c r; r.a = make_float2(v.x, v.y); r.b = make_float2(v.z, v.w); return r;
+#else
+  float4c r; r.a = p[0]; r.b = p[1]; return r;
+#endif
+}
+
 // C: partial sum of one thread: bin pair at k, partitions pg, pg + PG, ...; partition 0 from xnew, partition 1 from
-// xprev unless it is nullptr (then from the timeline like the rest)
+// xprev unless it is nullptr (then from the timeline like the rest).  kLive: timeline rows may have been stored earlier
+// in the same launch (step form), read them coherently.
+template <bool kLive = false>
 PC_HD float4c rt_sweep_thread(const RtParams& P, long long head, int c, int k, int pg, int PG, const float2* xnew,
                               const float2* xprev) {
   const float2* Hk = P.H + (long long)c * P.h_cstride + k;
@@ -171,7 +235,7 @@ PC_HD float4c rt_sweep_thread(const RtParams& P, long long head, int c, int k, i
         h[u] = ld_pair(Hk + (long long)pp * P.M);
         if (pp == 0) { x[u].a = xnew[k]; x[u].b = xnew[k + 1]; }
         else if (pp == 1 && xprev) { x[u].a = xprev[k]; x[u].b = xprev[k + 1]; }
-        else x[u] = ld_pair(Xk - (long long)pp * P.M);
+        else x[u] = kLive ? ld_pair_live(Xk - (long long)pp * P.M) : ld_pair(Xk - (long long)pp * P.M);
       } else {
         h[u].a = h[u].b = x[u].a = x[u].b = make_float2(0.f, 0.f);
       }
@@ -207,6 +271,8 @@ PC_D void rt_cluster_sync() {
 // the wait is free by then).
 PC_D void rt_cluster_arrive() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
 PC_D void rt_cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+// step form: a CTA done with a step's shared rows and timeline stores arrives; the next step's phase D waits
+PC_D void rt_cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
 // generic address of `p` (own shared memory) in CTA `rank` of the cluster
 template <class T>
 PC_D T* rt_map_rank(T* p, unsigned rank) {
@@ -262,10 +328,26 @@ __global__ void __launch_bounds__(256) k_rt_group(const __grid_constant__ RtGrou
   const int rank = blockIdx.x % cs;
 #include "kernels_rt_step.inc"
 }
+
+// The device-buffer group calls (b200conv_group_process_device, b200conv_chain_group_process_device): cluster i walks
+// member G.p[i]'s whole call of up to kRtMaxSteps head blocks (step form, RtStepParams); grid and cluster as k_rt_group.
+// No completion word: the caller orders its work on the stream.
+template <int M>
+__global__ void __launch_bounds__(256) k_rt_group_steps(const __grid_constant__ RtStepGroupParams G) {
+  const int cs = G.p[0].p.C * G.p[0].p.NC;
+  const RtStepParams& T = G.p[blockIdx.x / cs];
+  const RtParams& P = T.p;
+  const int rank = blockIdx.x % cs;
+#define PC_RT_STEPS
+#include "kernels_rt_step.inc"
+#undef PC_RT_STEPS
+}
 #else
 // CPU emulation (tests/emu): the CTAs of the cluster run phase by phase; a DSMEM store is a store into the other
 // CTA's arrays
-inline void emu_rt_block(const RtParams& P) {
+// T (step form): the call's segments are its step walk, the rows of xnew / yfull alternate, and every step is mixed
+// down before the next one
+inline void emu_rt_walk(const RtParams& P, const RtStepParams* T) {
   const int M = P.M, n = P.C * P.NC;
   const int MB = rt_row(M);
   struct Cta { float2 *bufA, *bufB, *xnew, *yfull; float *xs, *ys, *mix; float4* red; };
@@ -274,14 +356,16 @@ inline void emu_rt_block(const RtParams& P) {
     ct[r].bufA = new float2[MB]; ct[r].bufB = new float2[MB]; ct[r].xnew = new float2[2 * MB]; ct[r].yfull = new float2[2 * MB];
     ct[r].xs = new float[M]; ct[r].ys = new float[M]; ct[r].mix = new float[(size_t)P.C * M]; ct[r].red = new float4[256];
   }
-  for (int g = 0; g < P.nseg; ++g) {
-    const RtSeg& S = P.seg[g];
+  const int nseg = T ? rt_step_count(*T) : P.nseg;
+  for (int g = 0; g < nseg; ++g) {
+    const RtSeg S = T ? rt_step_seg(*T, g) : P.seg[g];
+    const int row = g & 1, prev = (g + 1) & 1;
     // A + B (each phase runs over every CTA before the next, so the second segment's stores into the open block
     // follow every CTA's reads of the first)
     for (int r = 0; r < n && P.mode != 2; ++r) {
       const int c = r / P.NC, q = r % P.NC;
       Cta& t = ct[r];
-      float2* xnew = t.xnew + g * MB;
+      float2* xnew = t.xnew + row * MB;
       for (int i = 0; i < M; ++i) rt_assemble(P, S, c, q, i, t.xs);
       float2* res = t.bufA;
       if (M == 1) {
@@ -313,7 +397,7 @@ inline void emu_rt_block(const RtParams& P) {
       for (int tid = 0; tid < 256; ++tid) {
         const int pi = tid % pairs, pg = tid / pairs, k = q * (M / P.NC) + 2 * pi;
         if (pg < PG) {
-          const float4c v = rt_sweep_thread(P, S.head, c, k, pg, PG, t.xnew + g * MB, g ? t.xnew : nullptr);
+          const float4c v = rt_sweep_thread(P, S.head, c, k, pg, PG, t.xnew + row * MB, g ? t.xnew + prev * MB : nullptr);
           t.red[tid].x = v.a.x; t.red[tid].y = v.a.y; t.red[tid].z = v.b.x; t.red[tid].w = v.b.y;
         }
       }
@@ -321,7 +405,7 @@ inline void emu_rt_block(const RtParams& P) {
         float4 v = t.red[tid];
         for (int gg = 1; gg < PG; ++gg) { const float4 u = t.red[tid + gg * pairs]; v.x += u.x; v.y += u.y; v.z += u.z; v.w += u.w; }
         const int k = q * (M / P.NC) + 2 * tid;
-        float2* dst = ct[c * P.NC].yfull + g * MB;
+        float2* dst = ct[c * P.NC].yfull + row * MB;
         dst[k] = make_float2(v.x, v.y); dst[k + 1] = make_float2(v.z, v.w);
         if (S.complete) {
           float2* yn = P.Ynext + (long long)c * P.y_cstride + k;
@@ -332,8 +416,8 @@ inline void emu_rt_block(const RtParams& P) {
     // E
     for (int c = 0; c < P.C && P.mode != 1; ++c) {
       Cta& t = ct[c * P.NC];
-      const float2* Yp = g ? t.yfull : P.Yprev + (long long)c * P.y_cstride;
-      const float2* Yt_src = t.yfull + g * MB;
+      const float2* Yp = g ? t.yfull + prev * MB : P.Yprev + (long long)c * P.y_cstride;
+      const float2* Yt_src = t.yfull + row * MB;
       if (P.mode == 2) {
         Yt_src = P.Yt + (long long)c * P.y_cstride;
         if (S.complete) for (int k = 0; k < M; ++k) P.Ynext[(long long)c * P.y_cstride + k] = Yt_src[k];
@@ -358,20 +442,23 @@ inline void emu_rt_block(const RtParams& P) {
       }
       for (int i = 0; i < S.len; ++i) {
         const float v = rt_out_sample(P, S, c, t.ys, S.fill + i);
-        if (P.mix_on) ct[0].mix[(size_t)c * M + S.off + i] = v; else P.out[(long long)c * P.out_stride + S.off + i] = v;
+        const int at = T ? i : S.off + i;
+        if (P.mix_on) ct[0].mix[(size_t)c * M + at] = v; else P.out[(long long)c * P.out_stride + S.off + i] = v;
       }
     }
-  }
-  if (P.mix_on && P.mode != 1)
-    for (int o = 0; o < P.n_out; ++o)
-      for (int i = 0; i < P.len; ++i) {
-        float acc = 0.0f;
-        for (int cc = 0; cc < P.C; ++cc) {
-          const float mm = P.mix[o * P.C + cc];
-          if (mm != 0.0f) acc = fmaf(mm, ct[0].mix[(size_t)cc * M + i], acc);
+    // the mixdown: after every step of the step form, after the last segment otherwise
+    const int mlen = T ? S.len : P.len, moff = T ? S.off : 0;
+    if (P.mix_on && P.mode != 1 && (T || g + 1 == nseg))
+      for (int o = 0; o < P.n_out; ++o)
+        for (int i = 0; i < mlen; ++i) {
+          float acc = 0.0f;
+          for (int cc = 0; cc < P.C; ++cc) {
+            const float mm = P.mix[o * P.C + cc];
+            if (mm != 0.0f) acc = fmaf(mm, ct[0].mix[(size_t)cc * M + i], acc);
+          }
+          P.out[(long long)o * P.out_stride + moff + i] = acc;
         }
-        P.out[(long long)o * P.out_stride + i] = acc;
-      }
+  }
   if (P.done_flag && P.mode != 1) *P.done_flag = P.done_val;
   for (int r = 0; r < n; ++r) {
     delete[] ct[r].bufA; delete[] ct[r].bufB; delete[] ct[r].xnew; delete[] ct[r].yfull;
@@ -380,9 +467,14 @@ inline void emu_rt_block(const RtParams& P) {
   delete[] ct;
 }
 
+inline void emu_rt_block(const RtParams& P) { emu_rt_walk(P, nullptr); }
+
 // the clusters of a group launch one after the other
 inline void emu_rt_group(const RtGroupParams& G) {
   for (int i = 0; i < G.n; ++i) emu_rt_block(G.p[i]);
+}
+inline void emu_rt_group_steps(const RtStepGroupParams& G) {
+  for (int i = 0; i < G.n; ++i) emu_rt_walk(G.p[i].p, &G.p[i]);
 }
 #endif
 
