@@ -43,7 +43,8 @@ typedef struct b200conv_config {
   int shard_count;       /* number of shards (1 = unsharded)                                        */
   int cmac_variant;      /* 0 = auto; >0 selects a specific CMAC kernel variant (tuning/bench):     */
                          /* 22 packed-FMA batched, 40 tensor cores (wgmma),   100..108 streaming,   */
-                         /* 41 line FFTs along the block index (overlap-save, FP32)                 */
+                         /* 41 line FFTs along the block index (overlap-save, FP32),                */
+                         /* 42 four-step 2^21-point FFTs of the samples (overlap-save, FP32)        */
 } b200conv_config;
 
 /* Lifetime ------------------------------------------------------------------------------- */
@@ -251,7 +252,10 @@ size_t b200conv_ir_len(const b200conv_t* h, int channel);    /* post-trim tap co
 unsigned long long b200conv_launch_count(const b200conv_t* h);
 /* Form of the FDL sweep (FFTConvolver.cpp:176-187) the last launch resolved to: 22 / 26 = packed-FMA batched sweep,
  * 40 = tensor-core sweep (wgmma f16, 3xFP16 with power-of-two scales), 41 = line-FFT sweep (4096-point FP32 overlap-save along
- * the block index, kernels_lfft.cuh), 100..108 = streaming forms.  For benchmarks and tests. */
+ * the block index, kernels_lfft.cuh), 42 = four-step sweep (2^21-point FP32 overlap-save of the samples themselves, in place
+ * of the group's forward FFT, sweep and inverse FFT, kernels_fourstep.cuh; whole-block, block-aligned B = 512 groups of an
+ * unsharded single-stage handle with at most 961 partitions; a forced 42 on any other shape is B200CONV_EINVAL),
+ * 100..108 = streaming forms.  For benchmarks and tests. */
 int b200conv_last_sweep_variant(const b200conv_t* h);
 /* Tuning / A-B switches: "rt" (1 = real-time calls of at most one head block run as ONE cluster-kernel launch
  * with zero-copy I/O, see b200conv_process; 0 = multi-kernel path), "fft512" (1 = register-resident FFT kernels for block size 512),
@@ -260,7 +264,9 @@ int b200conv_last_sweep_variant(const b200conv_t* h);
  * but 0 of a steady batch job — until the next b200conv_clear), "stream_alternate" (default 1: the streaming sweep
  * walks its partition slices in alternating directions from launch to launch, see kernels_stream.cuh), "tc" (default 1:
  * launch groups of >= 4096 blocks with <= 961 partitions run the sweep on the tensor cores, kernels_tc.cuh, and groups of
- * >= 16384 such blocks as FFT convolutions along the block index, kernels_lfft.cuh; 0 = always the packed-FMA sweep).
+ * >= 16384 such blocks as FFT convolutions along the block index, kernels_lfft.cuh, and B = 512 groups of >= 32768 blocks
+ * that qualify for it (see b200conv_last_sweep_variant) as four-step FFT convolutions of the samples, kernels_fourstep.cuh;
+ * 0 = always the packed-FMA sweep).
  * "shard_head" (sharded handles; set before b200conv_init_*, B200CONV_ESTATE once an IR is loaded; default 1 = every
  * stage partition-range sharded): 0 = tail layout — shard 0 holds the head stage (stage 0) whole and keeps the one-launch
  * real-time call, the other shards hold none of it (no head FFT, sweep or output, only the input buffering of the

@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200conv.so")
 SOURCES = ["engine.cu", "irshape.cu"]
-DEPS = ["engine.cu", "irshape.cu", "kernels.cuh", "kernels_stream.cuh", "kernels_fft512.cuh", "kernels_rt.cuh", "kernels_rt_step.inc", "kernels_chain.cuh", "kernels_chain_send.inc", "kernels_tc.cuh", "kernels_lfft.cuh",
+DEPS = ["engine.cu", "irshape.cu", "kernels.cuh", "kernels_stream.cuh", "kernels_fft512.cuh", "kernels_rt.cuh", "kernels_rt_step.inc", "kernels_chain.cuh", "kernels_chain_send.inc", "kernels_tc.cuh", "kernels_lfft.cuh", "kernels_fourstep.cuh",
         os.path.join("..", "..", "include", "b200conv.h")]
 
 NVCC_FLAGS = [

@@ -45,6 +45,7 @@
 #include "kernels_chain.cuh"
 #include "kernels_tc.cuh"
 #include "kernels_lfft.cuh"
+#include "kernels_fourstep.cuh"
 
 namespace {
 
@@ -236,6 +237,17 @@ struct b200conv {
   const void* lf_S_for = nullptr;
   int lf_S_P = 0, lf_S_B = 0, lf_S_C = 0;
   size_t lf_S_bytes = 0;
+  // four-step sweep (kernels_fourstep.cuh): the IR spectrum (cached like lf_S), the column spectra of a group, and the
+  // taps / the history in front of a group
+  float2* fs_S = nullptr;
+  const void* fs_S_for = nullptr;
+  int fs_S_P = 0, fs_S_B = 0, fs_S_C = 0;
+  size_t fs_S_bytes = 0;
+  float2* fs_X = nullptr;
+  size_t fs_X_bytes = 0;
+  float* fs_hist = nullptr;
+  size_t fs_hist_bytes = 0;
+  bool fs_attr_set = false;
   bool tc_alloc_failed = false;      // the scratch did not fit once: stay on the FFMA sweep
   int last_variant = 0;              // sweep form the last launch_cmac resolved to (b200conv_last_sweep_variant)
   // slot exchange (fused multi-GPU path), stage 0 of a single-stage handle
@@ -423,6 +435,9 @@ void free_all(b200conv* h) {
   h->tc_A = h->tc_Xt = nullptr; h->tc_Yt = nullptr; h->tc_A_for = nullptr; h->tc_A_bytes = h->tc_Xt_bytes = h->tc_Yt_bytes = 0;
   cudaFree(h->lf_S);
   h->lf_S = nullptr; h->lf_S_for = nullptr; h->lf_S_bytes = 0;
+  cudaFree(h->fs_S); cudaFree(h->fs_X); cudaFree(h->fs_hist);
+  h->fs_S = nullptr; h->fs_S_for = nullptr; h->fs_S_bytes = 0;
+  h->fs_X = nullptr; h->fs_X_bytes = 0; h->fs_hist = nullptr; h->fs_hist_bytes = 0;
   if (h->tc_err) cudaFreeHost(h->tc_err);
   h->tc_err = h->tc_err_dev = nullptr; h->tc_alloc_failed = false;
   h->route_in_only = false;
@@ -854,6 +869,8 @@ constexpr int kTcMinBlocks = 4096;      // below that a 128-segment tile is most
 // from here on the line-FFT sweep (kernels_lfft.cuh) replaces the tensor-core one; between the two thresholds the
 // Toeplitz form stays (its crossover with the line FFTs is not settled below this length)
 constexpr int kLfftMinBlocks = 16384;
+// from here on the four-step sweep (kernels_fourstep.cuh) replaces the line FFTs for the groups it takes
+constexpr int kFourStepMinBlocks = 32768;
 
 // can this sweep run on the tensor cores?  (geometry only; the scratch is allocated by launch_cmac_tc)
 bool tc_eligible(const b200conv* h, const pc::CmacParams& P, int C) {
@@ -909,6 +926,22 @@ bool tc_reserve_all(b200conv* h, const pc::CmacParams& P, int C, int variant, fl
   if (h->tc_A_for != P.H || h->tc_A_P != P.Ppad || h->tc_A_B != P.B || h->tc_A_C != C || h->tc_A_bytes < a_bytes) {
     h->tc_A_for = nullptr;
     if (!tc_reserve(h, &h->tc_A, &h->tc_A_bytes, a_bytes)) return false;
+  }
+  return true;
+}
+#endif
+
+#if !defined(PC_EMULATE)
+// the scratch of a four-step (42) group: column spectra, history and IR spectrum; false: not enough memory
+bool fs_reserve(b200conv* h, const pc::CmacParams& P, int C) {
+  namespace fs = pc::fs;
+  const fs::Plan plan = fs::make_plan(P.Ppad, (long long)P.nblocks * P.B);
+  if (!tc_reserve(h, &h->fs_X, &h->fs_X_bytes, fs::work_bytes(plan, C))) return false;
+  if (!tc_reserve(h, &h->fs_hist, &h->fs_hist_bytes, fs::hist_bytes(P.Ppad, C))) return false;
+  const size_t s_bytes = fs::spectrum_bytes(C);
+  if (h->fs_S_for != P.H || h->fs_S_P != P.Ppad || h->fs_S_B != P.B || h->fs_S_C != C || h->fs_S_bytes < s_bytes) {
+    h->fs_S_for = nullptr;
+    if (!tc_reserve(h, &h->fs_S, &h->fs_S_bytes, s_bytes)) return false;
   }
   return true;
 }
@@ -1010,27 +1043,40 @@ int launch_cmac_lfft(b200conv* h, const pc::CmacParams& P, int C, const TcDirect
 #endif
 }
 
+// streaming sweep of one block: 12 stages x 1 CTA/SM for rows below 512 bins and single-tile shapes of at most 32 MB,
+// which stay resident in the 50 MB L2 (fewer CTAs to ramp up); 6 stages x 2 CTAs/SM beyond
+int stream_variant(const pc::CmacParams& P, int C) {
+  const size_t bytes = (size_t)P.Ppad * P.B * 16 * (size_t)C;
+  return (P.B < 512 || (P.B == 512 && bytes <= (size_t)32 << 20)) ? 104 : 103;
+}
+
 // The sweep form of a launch (*variant).  A launch group decides it before its forward FFT: the tensor-core form
 // reserves its scratch here, so that when the memory is not there the FFMA sweep still finds the X rows it reads.
 // yc: where the tensor-core result lines go (the B = 512 direct form); nullptr: the handle's lines merged into Y rows.
+// fs_ok: the launch group may run as a four-step group (fourstep_ok).
 // P.Ppad enters as the number of real (unpadded) partition rows of this shard
-int select_cmac(b200conv* h, const pc::CmacParams& P, int C, float2** yc, size_t* yc_bytes, int* variant_out) {
+int select_cmac(b200conv* h, const pc::CmacParams& P, int C, float2** yc, size_t* yc_bytes, int* variant_out,
+                bool fs_ok = false) {
   int variant = h->cfg.cmac_variant;
   if (P.xg > 0) variant = (P.nblocks >= 64) ? 22 : 26;     // slot exchange: only the packed-FMA sweeps carry the exchange epilogue
   if (variant == 0) {
     // streaming sweep for real-time calls; packed-FMA batched sweep otherwise (TT = 16 when the
     // launch group is long enough to fill 16-block tiles, TT = 8 below that)
-    if (P.nblocks == 1 && P.B >= 64 && P.Ppad >= 1) {
-      // TMA ring: 6 stages x 2 CTAs/SM for working sets beyond L2 and multi-tile rows; 12 stages x 1 CTA/SM for rows
-      // below 512 bins and single-tile shapes of at most 32 MB, which stay resident in the 50 MB L2 (fewer CTAs to ramp up)
-      const size_t bytes = (size_t)P.Ppad * P.B * 16 * (size_t)C;
-      variant = (P.B < 512 || (P.B == 512 && bytes <= (size_t)32 << 20)) ? 104 : 103;
-    }
+    if (P.nblocks == 1 && P.B >= 64 && P.Ppad >= 1) variant = stream_variant(P, C);   // TMA ring
     else if (P.nblocks <= kStreamNBS && P.B >= 64 && P.Ppad >= 1) variant = 101;
     else if (P.nblocks <= kStreamNBS && P.B >= 2 && P.Ppad >= 1) variant = 100;
     else if (h->opt_tc && !h->tc_alloc_failed && P.nblocks >= kTcMinBlocks && tc_eligible(h, P, C))
-      variant = P.nblocks >= kLfftMinBlocks ? 41 : 40;
+      variant = fs_ok && P.nblocks >= kFourStepMinBlocks ? 42 : P.nblocks >= kLfftMinBlocks ? 41 : 40;
     else variant = (P.nblocks >= 64) ? 22 : 26;
+  }
+  if (variant == 42) {                         // four-step FFTs of the samples
+    if (!fs_ok) return fail(h, B200CONV_EINVAL, "four-step sweep: unsupported launch group (needs whole blocks from a block boundary, B = 512, at most 961 partitions, an unsharded single-stage handle)");
+#if !defined(PC_EMULATE)
+    if (!fs_reserve(h, P, C)) {
+      if (h->cfg.cmac_variant == 42) return fail(h, B200CONV_ENOMEM, "four-step sweep: scratch allocation failed");
+      variant = 41;                            // then the line FFTs, and below them the FFMA sweep
+    }
+#endif
   }
   if (variant == 40 || variant == 41) {        // wgmma 3xFP16 block-Toeplitz sweep / FP32 line FFTs
     if (!tc_eligible(h, P, C)) return fail(h, B200CONV_EINVAL, "tensor-core / line-FFT sweep: unsupported shape (needs B % 32 == 0, at most 961 partitions, no slot exchange)");
@@ -1890,6 +1936,105 @@ int run_group_p2p(b200conv* h, const float* in_dev, size_t in_stride, float* out
 int drain_tail(b200conv* h);
 int join_post(b200conv* h);
 
+// Can this launch group of stage s run as four-step FFT convolutions of its samples (variant 42)?  extra: the sweep
+// would start early (a time-slice rank's overlap state)
+bool fourstep_ok(const b200conv* h, const Stage& s, const Intake& it, int extra, int C) {
+#if defined(PC_EMULATE)
+  (void)h; (void)s; (void)it; (void)extra; (void)C;
+  return false;
+#else
+  return h->cfg.shard_count == 1 && h->stages.size() == 1 && extra == 0 && s.fill == 0 && it.partial == 0 &&
+         it.complete > 0 && pc::fs::plan_ok(s.P) && use_fft512(h, s.B, it.complete, C, s.tab512);
+#endif
+}
+
+// A four-step group (kernels_fourstep.cuh) in place of forward FFT, sweep and inverse FFT: history from the X rows in
+// front of the group, passes 1 and 2 on s_main, pass 3 into the output on ps.  Then the handle is left as a
+// line-FFT group leaves it: the X rows of the last s.hist blocks, and row 0 of the next Y buffer = sum_p H[p] X[last - p]
+// (a one-block streaming sweep), so that any form can follow.  The scratch is in place (fs_reserve).
+int run_group_fourstep(b200conv* h, Stage& s, const Intake& it, float* out_dev, size_t out_stride, size_t n, bool overlap) {
+#if defined(PC_EMULATE)
+  (void)s; (void)it; (void)out_dev; (void)out_stride; (void)n; (void)overlap;
+  return fail(h, B200CONV_EINVAL, "the four-step sweep is not part of the CPU emulation");
+#else
+  namespace fs = pc::fs;
+  const int C = h->C, B = s.B, P = s.P, complete = it.complete;
+  const fs::Plan plan = fs::make_plan(P, (long long)n);
+  const long long hl = (long long)P * B;
+  const int yb = s.ybuf, nxt = overlap ? (yb ^ 1) : yb;
+  cudaStream_t st = h->s_launch, ps = overlap ? h->s_post : st;
+  if (!h->fs_attr_set) {
+    CU_CHECK(h, cudaFuncSetAttribute(fs::k_fs_cols, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fs::kColSmem));
+    CU_CHECK(h, cudaFuncSetAttribute(fs::k_fs_cols_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fs::kColSmem));
+    h->fs_attr_set = true;
+  }
+  // the previous groups' post work may still read the column spectra (a four-step pass 3) and Y[nxt] row 0
+  if (overlap) {
+    CU_CHECK(h, cudaStreamWaitEvent(st, s.ev_post[0], 0));
+    CU_CHECK(h, cudaStreamWaitEvent(st, s.ev_post[1], 0));
+  }
+  const dim3 taps_block(32, 8), cols_grid(fs::kN2 / fs::kCols, plan.nseg, C);
+  if (h->fs_S_for != s.H || h->fs_S_P != P || h->fs_S_B != B || h->fs_S_C != C) {   // once per IR: taps -> spectrum
+    int id = timing_begin(h, kKindCmac);
+    fs::k_fs_taps<<<dim3((P + 7) / 8, C), taps_block, kF512Smem, st>>>(
+        fs::TapsParams{s.H, (long long)s.Prows * B, P, h->fs_hist, hl}, s.tab512);
+    fs::ColsParams tp{};
+    tp.src = h->fs_hist; tp.src_cstride = hl; tp.nsrc = hl; tp.nseg = 1; tp.dst = h->fs_S;
+    fs::k_fs_cols<<<dim3(fs::kN2 / fs::kCols, 1, C), fs::kColThreads, fs::kColSmem, st>>>(tp, s.tab512);
+    fs::k_fs_rows<false><<<C * fs::kRows, pc::lfft::kThreads, 0, st>>>(fs::RowsParams{h->fs_S, nullptr, 1});
+    timing_end(h, id);
+    h->fs_S_for = s.H; h->fs_S_P = P; h->fs_S_B = B; h->fs_S_C = C;
+    h->launches += 3;
+  }
+  // pass 1, its negative positions from the X rows [head - P, head)
+  int id = timing_begin(h, kKindFft);
+  fs::k_fs_taps<<<dim3((P + 7) / 8, C), taps_block, kF512Smem, st>>>(
+      fs::TapsParams{s.X + (s.head - P) * B, (long long)s.R * B, P, h->fs_hist, hl}, s.tab512);
+  fs::ColsParams cp{};
+  cp.src = it.src; cp.src_cstride = (long long)it.src_stride;
+  cp.use_cmap = (h->route_on || h->route_in_only) ? 1 : 0;
+  for (int c = 0; c < 8; ++c) cp.cmap[c] = h->in_map[c];
+  cp.nsrc = (long long)n; cp.hist = h->fs_hist; cp.hist_len = hl;
+  cp.w0 = fs::window_start(plan, 0); cp.L = plan.L; cp.nseg = plan.nseg; cp.dst = h->fs_X;
+  fs::k_fs_cols<<<cols_grid, fs::kColThreads, fs::kColSmem, st>>>(cp, s.tab512);
+  timing_end(h, id);
+  id = timing_begin(h, kKindCmac);
+  fs::k_fs_rows<true><<<(unsigned)(C * fs::kRows * plan.nseg), pc::lfft::kThreads, 0, st>>>(fs::RowsParams{h->fs_X, h->fs_S, plan.nseg});
+  timing_end(h, id);
+  h->launches += 3;
+  CU_CHECK(h, cudaGetLastError());
+  CU_CHECK(h, cudaEventRecord(s.ev_sweep[yb], st));
+  if (overlap) CU_CHECK(h, cudaStreamWaitEvent(ps, s.ev_sweep[yb], 0));
+
+  // pass 3 into the output (through the mixdown with routing on)
+  id = timing_begin(h, kKindIfft, ps);
+  const fs::ColsInvParams ip{h->fs_X, plan.nseg, plan, h->route_on ? h->dch[0] : out_dev,
+                             h->route_on ? (long long)h->Lmax : (long long)out_stride};
+  fs::k_fs_cols_inv<<<cols_grid, fs::kColThreads, fs::kColSmem, ps>>>(ip, s.tab512);
+  timing_end(h, id, ps);
+  h->launches++;
+  CU_CHECK(h, cudaGetLastError());
+  if (h->route_on) { if (int rc = launch_mix(h, h->dch[0], h->Lmax, out_dev, out_stride, n, ps)) return rc; }
+  if (overlap) CU_CHECK(h, cudaEventRecord(s.ev_post[yb], ps));
+
+  // the state every other form reads: the X rows of the last s.hist blocks ...
+  const int from = std::max(0, complete - s.hist);
+  pc::FwdParams fp = fwd_params(h, s, it.src + (size_t)from * B, it.src_stride, (long long)(complete - from) * B,
+                                complete - from, it.direct);
+  fp.dst_row0 = s.head + from;
+  if (int rc = launch_fwd(h, fp, C)) return rc;
+  // ... and the overlap state of the next group, the spectrum of the last block
+  pc::CmacParams op = sweep_params(s, C, s.Y[nxt], 1);
+  op.xrow0 = s.head + complete - 1;
+  op.yrow0 = 0;
+  if (int rc = launch_cmac_as(h, op, C, stream_variant(op, C), nullptr)) return rc;
+  s.ybuf = nxt;
+  s.head += complete;
+  s.blocks_done += complete;
+  return 0;
+#endif
+}
+
 // `overlap`: reduce + inverse FFT go to s_post so that they overlap the next group's forward
 // FFT + sweep on s_main (double-buffered Y); otherwise everything is issued on s_main.
 int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev, size_t out_stride, size_t n,
@@ -1936,7 +2081,13 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
       const pc::CmacParams cp = sweep_params(s, C, Yb, nb, extra);
       const bool direct_ok = h->cfg.shard_count == 1 && use_fft512(h, B, nb, C, s.tab512);
       int variant = 0;
-      if (int rc = select_cmac(h, cp, C, direct_ok ? &s.tcY[yb] : nullptr, &s.tcY_bytes[yb], &variant)) return rc;
+      if (int rc = select_cmac(h, cp, C, direct_ok ? &s.tcY[yb] : nullptr, &s.tcY_bytes[yb], &variant,
+                               si == 0 && fourstep_ok(h, s, it, extra, C))) return rc;
+      if (variant == 42) {
+        if (int rc = run_group_fourstep(h, s, it, out_dev, out_stride, n, overlap)) return rc;
+        if (int rc = intake_end(h, s, it)) return rc;
+        continue;
+      }
       tc_direct = direct_ok && (variant == 40 || variant == 41);
 
       pc::FwdParams fp = fwd_params(h, s, it.src, it.src_stride, (long long)it.total, nb, it.direct);
