@@ -248,6 +248,7 @@ struct b200conv {
   float* fs_hist = nullptr;
   size_t fs_hist_bytes = 0;
   bool fs_attr_set = false;
+  unsigned fs_rows_ctas[2] = {0, 0};  // resident CTAs of k_fs_rows<false> / <true> on the device (persistent grid)
   bool tc_alloc_failed = false;      // the scratch did not fit once: stay on the FFMA sweep
   int last_variant = 0;              // sweep form the last launch_cmac resolved to (b200conv_last_sweep_variant)
   // slot exchange (fused multi-GPU path), stage 0 of a single-stage handle
@@ -1966,6 +1967,16 @@ int run_group_fourstep(b200conv* h, Stage& s, const Intake& it, float* out_dev, 
   if (!h->fs_attr_set) {
     CU_CHECK(h, cudaFuncSetAttribute(fs::k_fs_cols, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fs::kColSmem));
     CU_CHECK(h, cudaFuncSetAttribute(fs::k_fs_cols_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fs::kColSmem));
+    CU_CHECK(h, cudaFuncSetAttribute(fs::k_fs_rows<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fs::rows_smem<false>()));
+    CU_CHECK(h, cudaFuncSetAttribute(fs::k_fs_rows<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fs::rows_smem<true>()));
+    int dev = 0, sms = 0, per_sm[2] = {0, 0};
+    CU_CHECK(h, cudaGetDevice(&dev));
+    CU_CHECK(h, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    CU_CHECK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[0], fs::k_fs_rows<false>, pc::lfft::kThreads, fs::rows_smem<false>()));
+    CU_CHECK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[1], fs::k_fs_rows<true>, pc::lfft::kThreads, fs::rows_smem<true>()));
+    if (per_sm[0] < 1 || per_sm[1] < 1) return fail(h, B200CONV_ECUDA, "the four-step row pass does not fit an SM");
+    h->fs_rows_ctas[0] = (unsigned)(per_sm[0] * sms);
+    h->fs_rows_ctas[1] = (unsigned)(per_sm[1] * sms);
     h->fs_attr_set = true;
   }
   // the previous groups' post work may still read the column spectra (a four-step pass 3) and Y[nxt] row 0
@@ -1981,7 +1992,9 @@ int run_group_fourstep(b200conv* h, Stage& s, const Intake& it, float* out_dev, 
     fs::ColsParams tp{};
     tp.src = h->fs_hist; tp.src_cstride = hl; tp.nsrc = hl; tp.nseg = 1; tp.dst = h->fs_S;
     fs::k_fs_cols<<<dim3(fs::kN2 / fs::kCols, 1, C), fs::kColThreads, fs::kColSmem, st>>>(tp, s.tab512);
-    fs::k_fs_rows<false><<<C * fs::kRows, pc::lfft::kThreads, 0, st>>>(fs::RowsParams{h->fs_S, nullptr, 1});
+    const unsigned items = (unsigned)(C * fs::kRows);
+    fs::k_fs_rows<false><<<std::min(items, h->fs_rows_ctas[0]), pc::lfft::kThreads, fs::rows_smem<false>(), st>>>(
+        fs::RowsParams{h->fs_S, nullptr, 1, items});
     timing_end(h, id);
     h->fs_S_for = s.H; h->fs_S_P = P; h->fs_S_B = B; h->fs_S_C = C;
     h->launches += 3;
@@ -1999,7 +2012,9 @@ int run_group_fourstep(b200conv* h, Stage& s, const Intake& it, float* out_dev, 
   fs::k_fs_cols<<<cols_grid, fs::kColThreads, fs::kColSmem, st>>>(cp, s.tab512);
   timing_end(h, id);
   id = timing_begin(h, kKindCmac);
-  fs::k_fs_rows<true><<<(unsigned)(C * fs::kRows * plan.nseg), pc::lfft::kThreads, 0, st>>>(fs::RowsParams{h->fs_X, h->fs_S, plan.nseg});
+  const unsigned items = (unsigned)(C * fs::kRows * plan.nseg);
+  fs::k_fs_rows<true><<<std::min(items, h->fs_rows_ctas[1]), pc::lfft::kThreads, fs::rows_smem<true>(), st>>>(
+      fs::RowsParams{h->fs_X, h->fs_S, plan.nseg, items});
   timing_end(h, id);
   h->launches += 3;
   CU_CHECK(h, cudaGetLastError());

@@ -24,7 +24,9 @@
 // movement.  Samples come in as 128-byte rows of 32 columns and column spectra leave as 256-byte rows: a shared-memory
 // tile transposes both ways, and doubles as the warps' exchange buffers.  Twiddles W_M^e: e = n2 k1 < 2^20, so
 // sincospif(e / 2^20) has an exact argument.
-// Row pass: kernels_lfft.cuh's 4096-point transform, pointwise product and conjugate inverse, 1 / M folded into S.
+// Row pass: kernels_lfft.cuh's 4096-point transform, pointwise product and conjugate inverse, 1 / M folded into S,
+// in persistent CTAs that walk contiguous ranges of the rows with the next row and the spectrum row bulk-copied into
+// shared memory.  Column spectra are [C][kRows][nseg][kN2]: the segments of a row are one contiguous run.
 //
 // k_fs_taps turns packed 1024-point spectrum rows back into their first 512 samples: the taps from the partition
 // spectra H (for the IR spectrum: taps, pass 1, pass 2 without the product), and the history in front of a group
@@ -63,6 +65,14 @@ PC_TC_HD Plan make_plan(int P, long long n) {
   return p;
 }
 PC_TC_HD bool plan_ok(int P) { return P >= 1 && P <= kMaxP; }
+// the items [begin, end) of CTA b of the persistent row pass: ctas contiguous ranges of items whose lengths differ by at
+// most one, so no range is longer than ceil(items / ctas)
+struct ItemRange {
+  unsigned begin, end;
+};
+PC_TC_HD ItemRange item_range(unsigned items, unsigned ctas, unsigned b) {
+  return ItemRange{(unsigned)((unsigned long long)items * b / ctas), (unsigned)((unsigned long long)items * (b + 1) / ctas)};
+}
 // first window sample (relative to the group's first sample) of segment q
 PC_TC_HD long long window_start(const Plan& p, int q) { return (long long)q * p.L - (p.Lh - 1); }
 // group output of window position m of segment q, or -1 (m < Lh - 1: the wrapped part; or past the group's end)
@@ -71,7 +81,8 @@ PC_TC_HD long long output_of(const Plan& p, int q, long long m) {
   const long long t = (long long)q * p.L + m - (p.Lh - 1);
   return t < p.n ? t : -1;
 }
-// the column spectra of every segment and channel, [C][nseg][kRows][kN2] complex
+// the column spectra of every segment and channel, [C][kRows][nseg][kN2] complex: the nseg segments of a row are one
+// contiguous run
 PC_TC_HD size_t work_bytes(const Plan& p, int C) { return (size_t)C * p.nseg * kRows * kN2 * 8; }
 // the IR spectrum in pass-2 layout, [C][kRows][kN2] complex
 PC_TC_HD size_t spectrum_bytes(int C) { return (size_t)C * kRows * kN2 * 8; }
@@ -139,7 +150,7 @@ struct ColsParams {
   long long hist_len;
   long long w0, L;          // segment q's window starts at position w0 + q L
   int nseg;
-  float2* dst;              // [C][nseg][kRows][kN2]
+  float2* dst;              // [C][kRows][nseg][kN2]
 };
 
 // grid (kN2 / kCols, nseg, C), block kColThreads, dynamic smem kColSmem
@@ -229,68 +240,113 @@ __global__ void __launch_bounds__(kColThreads, 2) k_fs_cols(ColsParams p, const 
     for (int q1 = 0; q1 < 4; ++q1) put(32 + 64 * q1, B[q1], B[7 - q1]);
   }
   __syncthreads();
-  float4* dst = reinterpret_cast<float4*>(p.dst + (((long long)c * p.nseg + q) * kRows) * kN2 + n2_0);
+  float4* dst = reinterpret_cast<float4*>(p.dst + ((long long)c * kRows * p.nseg + q) * kN2 + n2_0);
+  const long long rs4 = (long long)p.nseg * (kN2 / 2);       // row stride in float4
 #pragma unroll 3
   for (int e = tid; e < kRows * 16; e += kColThreads) {
     const int k1 = e >> 4, pr = e & 15, n2 = n2_0 + 2 * pr;
     const float4 s = st[k1 * kStage4 + pr];
     const float2 x0 = lfft::cmul(make_float2(s.x, s.y), wM(n2 * k1, false));
     const float2 x1 = lfft::cmul(make_float2(s.z, s.w), wM((n2 + 1) * k1, false));
-    dst[(long long)k1 * (kN2 / 2) + pr] = make_float4(x0.x, x0.y, x1.x, x1.y);
+    dst[k1 * rs4 + pr] = make_float4(x0.x, x0.y, x1.x, x1.y);
   }
 }
 
 // ---- pass 2 ---------------------------------------------------------------------------------------------------
 struct RowsParams {
-  float2* X;                // [C][nseg][kRows][kN2], in place
+  float2* X;                // [C][kRows][nseg][kN2], in place
   const float2* S;          // [C][kRows][kN2] (MUL)
   int nseg;
+  unsigned items;           // C * kRows * nseg: item i is row i of X, spectrum row i / nseg
 };
 
-// grid (C * kRows * nseg), block lfft::kThreads; item = (c * kRows + k1) * nseg + q, so that the segments of a row
-// follow each other and its spectrum row comes from L2.  MUL = false (the IR spectrum): the forward transform only,
-// stored times 1 / M
+// dynamic shared memory of the row pass: every thread's twiddle bases, the stage (the next item's row) and, for MUL,
+// the spectrum row
+template <bool MUL>
+constexpr size_t rows_smem() { return (size_t)(2 * lfft::kThreads + (MUL ? 2 : 1) * kN2) * sizeof(float2); }
+
+// lfft::fft4096 with thread j's twiddle bases read from tw[2 j], tw[2 j + 1] where each pass needs them: held in
+// registers across the loop of k_fs_rows, they would not fit its register budget
+__device__ __forceinline__ void fft4096_tw(float2 (&a)[16], float* sre, float* sim, int j, const float2* tw) {
+  lfft::dft16(a);
+  lfft::exchange<1>(a, sre, sim, j);
+  lfft::twiddle(a, tw[2 * j]);
+  lfft::dft16(a);
+  lfft::exchange<16>(a, sre, sim, j);
+  lfft::twiddle(a, tw[2 * j + 1]);
+  lfft::dft16(a);
+}
+
+// Persistent: grid = the resident CTAs (at most items), block lfft::kThreads, dynamic smem rows_smem<MUL>().  CTA b
+// walks item_range(items, gridDim.x, b) in order, so the resident CTAs move through one contiguous region of X and a
+// CTA's items share a spectrum row nseg at a time.  While item i is transformed, item i + 1's row is already on its way
+// into the stage by a bulk copy (`full` mbarrier); the spectrum row is bulk-copied into shared memory only when the
+// item's row k1 changes (`spec` mbarrier).  Each stage and spectrum copy is issued by thread 0 after a barrier that
+// follows every thread's last read of the previous content.  Results are stored from registers.  MUL = false (the IR
+// spectrum): the forward transform only, stored times 1 / M
 template <bool MUL>
 __global__ void __launch_bounds__(lfft::kThreads, 2) k_fs_rows(RowsParams p) {
   __shared__ float sre[lfft::kSmemFloats], sim[lfft::kSmemFloats];
+  __shared__ unsigned long long bar[2];             // full, spec
+  extern __shared__ __align__(128) float2 pc_smem_fs_rows[];
+  float2* tw = pc_smem_fs_rows;
+  float2* stage = pc_smem_fs_rows + 2 * lfft::kThreads;
+  float2* spec = stage + kN2;
+  constexpr unsigned kRowBytes = kN2 * sizeof(float2);
   const int j = threadIdx.x;
-  // (c * nseg + q) * kRows + k1 of item (c * kRows + k1) * nseg + q; recomputed where it is used, so that no
-  // pointer stays live across the transforms
-  auto row = [&]() {
-    const unsigned q = blockIdx.x % (unsigned)p.nseg, ck = blockIdx.x / (unsigned)p.nseg, c = ck / kRows;
-    return p.X + (((long long)c * p.nseg + q) * kRows + (ck - c * kRows)) * kN2;
-  };
-  float2 a[16];
-  {
-    const float2* x = row();
-#pragma unroll
-    for (int r = 0; r < 16; ++r) a[r] = x[j + 256 * r];
+  const ItemRange rg = item_range(p.items, gridDim.x, blockIdx.x);
+  if (rg.begin >= rg.end) return;
+  if (j == 0) {
+    tc::mbar_init(&bar[0], 1);
+    tc::mbar_init(&bar[1], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    tc::mbar_expect(&bar[0], kRowBytes);
+    tc::bulk_load(stage, p.X + (size_t)rg.begin * kN2, kRowBytes, &bar[0]);
   }
-  float2 tw1, tw2;
-  lfft::twiddle_bases(j, tw1, tw2);
-  lfft::fft4096(a, sre, sim, j, tw1, tw2);
-  if (MUL) {
-    const float2* S = p.S + (long long)(blockIdx.x / (unsigned)p.nseg) * kN2;
+  lfft::twiddle_bases(j, tw[2 * j], tw[2 * j + 1]);
+  __syncthreads();
+  unsigned srow = ~0u, nspec = 0;
+  for (unsigned i = rg.begin; i < rg.end; ++i) {
+    float2 a[16];
+    (void)tc::mbar_wait(&bar[0], (i - rg.begin) & 1u);
 #pragma unroll
-    for (int r = 0; r < 16; ++r) {
-      const float2 y = lfft::cmul(a[r], __ldg(S + j + 256 * r));
-      a[r] = make_float2(y.x, -y.y);                 // conj: the inverse as a forward transform
+    for (int r = 0; r < 16; ++r) a[r] = stage[j + 256 * r];
+    __syncthreads();                                // the stage and the previous item's spectrum row are read
+    const unsigned row = MUL ? i / (unsigned)p.nseg : 0u;
+    if (j == 0) {
+      if (i + 1 < rg.end) {
+        tc::mbar_expect(&bar[0], kRowBytes);
+        tc::bulk_load(stage, p.X + (size_t)(i + 1) * kN2, kRowBytes, &bar[0]);
+      }
+      if (MUL && row != srow) {
+        tc::mbar_expect(&bar[1], kRowBytes);
+        tc::bulk_load(spec, p.S + (size_t)row * kN2, kRowBytes, &bar[1]);
+      }
     }
-    lfft::fft4096(a, sre, sim, j, tw1, tw2);
-    float2* y = row();
+    if (MUL && row != srow) { srow = row; ++nspec; }
+    fft4096_tw(a, sre, sim, j, tw);
+    float2* y = p.X + (size_t)i * kN2;
+    if (MUL) {
+      (void)tc::mbar_wait(&bar[1], (nspec - 1) & 1u);
 #pragma unroll
-    for (int r = 0; r < 16; ++r) y[j + 256 * r] = make_float2(a[r].x, -a[r].y);
-  } else {
-    constexpr float inv_m = 1.0f / (float)kM;       // exact
-    float2* y = row();
+      for (int r = 0; r < 16; ++r) {
+        const float2 v = lfft::cmul(a[r], spec[j + 256 * r]);
+        a[r] = make_float2(v.x, -v.y);               // conj: the inverse as a forward transform
+      }
+      fft4096_tw(a, sre, sim, j, tw);
 #pragma unroll
-    for (int r = 0; r < 16; ++r) y[j + 256 * r] = make_float2(a[r].x * inv_m, a[r].y * inv_m);
+      for (int r = 0; r < 16; ++r) y[j + 256 * r] = make_float2(a[r].x, -a[r].y);
+    } else {
+      constexpr float inv_m = 1.0f / (float)kM;     // exact
+#pragma unroll
+      for (int r = 0; r < 16; ++r) y[j + 256 * r] = make_float2(a[r].x * inv_m, a[r].y * inv_m);
+    }
   }
 }
 
 // ---- pass 3 ---------------------------------------------------------------------------------------------------
 struct ColsInvParams {
-  const float2* X;          // [C][nseg][kRows][kN2] (pass 2)
+  const float2* X;          // [C][kRows][nseg][kN2] (pass 2)
   int nseg;
   Plan plan;
   float* dst;               // channel c: dst + c * dst_cstride, index t = group output t
@@ -304,14 +360,15 @@ __global__ void __launch_bounds__(kColThreads, 2) k_fs_cols_inv(ColsInvParams p,
   float2* buf = pc_smem_fs + kF512_TabLen;
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int n2_0 = blockIdx.x * kCols, q = blockIdx.y, c = blockIdx.z;
-  const float4* src = reinterpret_cast<const float4*>(p.X + (((long long)c * p.nseg + q) * kRows) * kN2 + n2_0);
+  const float4* src = reinterpret_cast<const float4*>(p.X + ((long long)c * kRows * p.nseg + q) * kN2 + n2_0);
+  const unsigned rs4 = (unsigned)p.nseg * (kN2 / 2);         // row stride in float4
   float4* st = reinterpret_cast<float4*>(buf);
   constexpr int kIt = (kRows * 16 + kColThreads - 1) / kColThreads;
   float4 v[kIt];
 #pragma unroll
   for (int i = 0; i < kIt; ++i) {
     const int e = tid + i * kColThreads;
-    if (e < kRows * 16) v[i] = __ldg(src + (long long)(e >> 4) * (kN2 / 2) + (e & 15));
+    if (e < kRows * 16) v[i] = __ldg(src + (size_t)((e >> 4) * rs4) + (e & 15));
   }
   for (int j = tid; j < kF512_TabLen; j += kColThreads) tab[j] = tab512[j];
 #pragma unroll
