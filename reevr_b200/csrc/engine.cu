@@ -58,6 +58,25 @@ constexpr int kMaxBlockLog2 = 13;     // B <= 8192 (two M-point ping-pong buffer
 inline size_t next_pow2(size_t v) { size_t p = 1; while (p < v) p *= 2; return p; }
 inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
+// grow-only device scratch of the long sweep forms (reserve)
+template <class T>
+struct Scratch {
+  T* p = nullptr;
+  size_t bytes = 0;
+  void release() { cudaFree(p); *this = Scratch(); }
+};
+
+// An operand a long sweep form builds once from one stage's partition spectra H and keeps until the IR changes
+template <class T>
+struct IrCache {
+  Scratch<T> buf;
+  const void* H = nullptr;           // the H (with its partition rows, block size and channels) it was built from
+  int P = 0, B = 0, C = 0;
+  bool holds(const pc::CmacParams& cp, int c) const { return H == cp.H && P == cp.Ppad && B == cp.B && C == c; }
+  void built_from(const pc::CmacParams& cp, int c) { H = cp.H; P = cp.Ppad; B = cp.B; C = c; }
+  void release() { buf.release(); H = nullptr; }
+};
+
 struct Stage {
   int B = 0;
   size_t tap_off = 0;      // first IR tap of this stage
@@ -77,8 +96,7 @@ struct Stage {
   float2* X = nullptr;
   float2* Y[2] = {nullptr, nullptr};   // double buffer: the sweep of group i+1 may overlap reduce+IFFT of group i
   // B = 512 groups on the tensor-core sweep: its bin-major complex result, read by the inverse FFT (paired with Y[b])
-  float2* tcY[2] = {nullptr, nullptr};
-  size_t tcY_bytes[2] = {0, 0};
+  Scratch<float2> tcY[2];
   int ybuf = 0;
   cudaEvent_t ev_sweep[2] = {nullptr, nullptr};   // Y[b] rows written by the sweep
   cudaEvent_t ev_post[2] = {nullptr, nullptr};    // Y[b] no longer needed by reduce / inverse FFT
@@ -223,33 +241,21 @@ struct b200conv {
   // tensor-core sweep (kernels_tc.cuh): Toeplitz tile images of one stage's H, per-bin time lines, the bin-major
   // complex result of the groups that merge it into Y rows
   bool opt_tc = std::getenv("B200CONV_NO_TC") == nullptr;
-  void* tc_A = nullptr;              // FP16 images, then the per-line scale exponents (kernels_tc.cuh a_image_bytes_gauss)
-  const void* tc_A_for = nullptr;    // H the images were built from (+ its geometry)
-  int tc_A_P = 0, tc_A_B = 0, tc_A_C = 0;
-  float* tc_Xt = nullptr;
-  float2* tc_Yt = nullptr;
-  size_t tc_A_bytes = 0, tc_Xt_bytes = 0, tc_Yt_bytes = 0;
+  IrCache<void> tc_A;                // FP16 images, then the per-line scale exponents (kernels_tc.cuh a_image_bytes_gauss)
+  Scratch<float> tc_Xt;
+  Scratch<float2> tc_Yt;
   int* tc_err = nullptr;             // mapped pinned word: a barrier wait of k_tc_sweep gave up
   int* tc_err_dev = nullptr;
-  bool tc_attr_set = false;
-  // line-FFT sweep (kernels_lfft.cuh): kN-point spectra of every line of one stage's H, cached like tc_A
-  float2* lf_S = nullptr;
-  const void* lf_S_for = nullptr;
-  int lf_S_P = 0, lf_S_B = 0, lf_S_C = 0;
-  size_t lf_S_bytes = 0;
-  // four-step sweep (kernels_fourstep.cuh): the IR spectrum (cached like lf_S), the column spectra of a group, and the
-  // taps / the history in front of a group
-  float2* fs_S = nullptr;
-  const void* fs_S_for = nullptr;
-  int fs_S_P = 0, fs_S_B = 0, fs_S_C = 0;
-  size_t fs_S_bytes = 0;
-  float2* fs_X = nullptr;
-  size_t fs_X_bytes = 0;
-  float* fs_hist = nullptr;
-  size_t fs_hist_bytes = 0;
-  bool fs_attr_set = false;
+  // line-FFT sweep (kernels_lfft.cuh): kN-point spectra of every line of one stage's H
+  IrCache<float2> lf_S;
+  // four-step sweep (kernels_fourstep.cuh): the IR spectrum, the column spectra of a group, and the taps / the history
+  // in front of a group
+  IrCache<float2> fs_S;
+  Scratch<float2> fs_X;
+  Scratch<float> fs_hist;
   unsigned fs_rows_ctas[2] = {0, 0};  // resident CTAs of k_fs_rows<false> / <true> on the device (persistent grid)
-  bool tc_alloc_failed = false;      // the scratch did not fit once: stay on the FFMA sweep
+  // the scratch of a long form (40, 41 or 42) did not fit once: automatic selection stays on the FFMA sweep
+  bool tc_alloc_failed = false;
   int last_variant = 0;              // sweep form the last launch_cmac resolved to (b200conv_last_sweep_variant)
   // slot exchange (fused multi-GPU path), stage 0 of a single-stage handle
   bool p2p_on = false;
@@ -338,7 +344,7 @@ int cuda_fail(b200conv* h, cudaError_t e, const char* what) {
 int fail(b200conv* h, int code, const std::string& msg) { h->err = msg; return code; }
 
 void free_stage(Stage& s) {
-  cudaFree(s.H); cudaFree(s.X); cudaFree(s.Y[0]); cudaFree(s.Y[1]); cudaFree(s.tcY[0]); cudaFree(s.tcY[1]); cudaFree(s.tw); cudaFree(s.tab512); cudaFree(s.inbuf); cudaFree(s.inbuf_alt); cudaFree(s.fut);
+  cudaFree(s.H); cudaFree(s.X); cudaFree(s.Y[0]); cudaFree(s.Y[1]); s.tcY[0].release(); s.tcY[1].release(); cudaFree(s.tw); cudaFree(s.tab512); cudaFree(s.inbuf); cudaFree(s.inbuf_alt); cudaFree(s.fut);
   for (int i = 0; i < 2; ++i) {
     if (s.ev_job[i]) cudaEventDestroy(s.ev_job[i]);
     if (s.ev_sweep[i]) cudaEventDestroy(s.ev_sweep[i]);
@@ -432,13 +438,8 @@ void free_all(b200conv* h) {
     h->din[i] = h->dout[i] = nullptr;
   }
   cudaFree(h->dch[0]); h->dch[0] = nullptr;
-  cudaFree(h->tc_A); cudaFree(h->tc_Xt); cudaFree(h->tc_Yt);
-  h->tc_A = h->tc_Xt = nullptr; h->tc_Yt = nullptr; h->tc_A_for = nullptr; h->tc_A_bytes = h->tc_Xt_bytes = h->tc_Yt_bytes = 0;
-  cudaFree(h->lf_S);
-  h->lf_S = nullptr; h->lf_S_for = nullptr; h->lf_S_bytes = 0;
-  cudaFree(h->fs_S); cudaFree(h->fs_X); cudaFree(h->fs_hist);
-  h->fs_S = nullptr; h->fs_S_for = nullptr; h->fs_S_bytes = 0;
-  h->fs_X = nullptr; h->fs_X_bytes = 0; h->fs_hist = nullptr; h->fs_hist_bytes = 0;
+  h->tc_A.release(); h->tc_Xt.release(); h->tc_Yt.release(); h->lf_S.release();
+  h->fs_S.release(); h->fs_X.release(); h->fs_hist.release();
   if (h->tc_err) cudaFreeHost(h->tc_err);
   h->tc_err = h->tc_err_dev = nullptr; h->tc_alloc_failed = false;
   h->route_in_only = false;
@@ -865,7 +866,21 @@ int launch_cmac_stream_tma(b200conv* h, const pc::CmacParams& P, int C, int stag
   return 0;
 }
 
-// ---- tensor-core sweep (kernels_tc.cuh) -------------------------------------------------------------------------
+// streaming sweep of one block: 12 stages x 1 CTA/SM for rows below 512 bins and single-tile shapes of at most 32 MB,
+// which stay resident in the 50 MB L2 (fewer CTAs to ramp up); 6 stages x 2 CTAs/SM beyond
+int stream_variant(const pc::CmacParams& P, int C) {
+  const size_t bytes = (size_t)P.Ppad * P.B * 16 * (size_t)C;
+  return (P.B < 512 || (P.B == 512 && bytes <= (size_t)32 << 20)) ? 104 : 103;
+}
+
+// the TMA streaming sweep of one block as form 102 - 105; xch: with the tail slot exchange epilogue (103 / 104)
+int launch_stream_ring(b200conv* h, const pc::CmacParams& P, int C, int variant, const TailXch* xch = nullptr) {
+  // 102: 4 stages x 3 CTAs/SM   103: 6 x 2   104: 12 x 1   105: 2 x 6    (all 192 KB in flight per SM)
+  static const int cfg[4][2] = {{4, 3}, {6, 2}, {12, 1}, {2, 6}};
+  return launch_cmac_stream_tma(h, P, C, cfg[variant - 102][0], cfg[variant - 102][1], false, -1.0f, xch);
+}
+
+// ---- the sweep form of a launch; long launch groups: tensor-core (40), line-FFT (41) and four-step (42) sweeps -------
 constexpr int kTcMinBlocks = 4096;      // below that a 128-segment tile is mostly padding: the FFMA sweep is faster
 // from here on the line-FFT sweep (kernels_lfft.cuh) replaces the tensor-core one; between the two thresholds the
 // Toeplitz form stays (its crossover with the line FFTs is not settled below this length)
@@ -873,101 +888,93 @@ constexpr int kLfftMinBlocks = 16384;
 // from here on the four-step sweep (kernels_fourstep.cuh) replaces the line FFTs for the groups it takes
 constexpr int kFourStepMinBlocks = 32768;
 
-// can this sweep run on the tensor cores?  (geometry only; the scratch is allocated by launch_cmac_tc)
-bool tc_eligible(const b200conv* h, const pc::CmacParams& P, int C) {
-#if defined(PC_EMULATE)
-  (void)h; (void)P; (void)C;
-  return false;
-#else
+// The sweep form select_cmac chose.  In the B = 512 direct form of a tensor-core or line-FFT launch group (run_group)
+// the sweep's bin-major complex result stays in yc for the inverse FFT, lines yc_stride apart; output 0 of the sweep
+// is block -extra of the group (extra = 1: the sweep computes the overlap state)
+struct Sweep {
+  int variant = 0;
+  float2* yc = nullptr;              // nullptr: the result lines are merged into Y rows
+  long long yc_stride = 0;
+  int extra = 0;
+};
+
+// How the n samples of a launch group enter a stage's open block: `complete` blocks to transform from `src`, `partial`
+// samples left over as the next open block.
+struct Intake { int complete, partial; bool direct; const float* src; size_t src_stride; size_t total; };
+// the launch-group helpers run_group_fourstep shares with run_group (defined with them below)
+pc::CmacParams sweep_params(const Stage& s, int C, float2* Y, int nblocks, int extra = 0);
+pc::FwdParams fwd_params(const b200conv* h, const Stage& s, const float* src, size_t src_stride, long long nvalid,
+                         int nblocks, bool direct);
+int launch_mix(b200conv* h, const float* in, size_t in_stride, float* out, size_t out_stride, size_t n, cudaStream_t st);
+
+#if !defined(PC_EMULATE)
+// can this sweep run on the tensor cores or the line FFTs?  (geometry only; the scratch is reserve_form's)
+bool tc_eligible(const pc::CmacParams& P, int C) {
   if (P.xg > 0 || P.Ppad < 1 || P.nblocks < 1) return false;
   const pc::tc::Geom g = pc::tc::make_geom(P.Ppad, P.nblocks);
   if (!pc::tc::geom_ok(g, P.B)) return false;
   return (unsigned long long)C * P.B * 4ull * (unsigned long long)g.rows < (1ull << 31);
-#endif
 }
 
-#if !defined(PC_EMULATE)
-// grow-only device scratch; a failed allocation is not an error of the call (the caller falls back to the FFMA sweep)
-template <typename T>
-bool tc_reserve(b200conv* h, T** buf, size_t* have, size_t need) {
-  if (*have >= need) return true;
-  cudaFree(*buf);
-  *buf = nullptr; *have = 0;
-  if (cudaMalloc((void**)buf, need) != cudaSuccess) { cudaGetLastError(); *buf = nullptr; h->tc_alloc_failed = true; return false; }
-  *have = need;
+// Can this launch group of stage s run as four-step FFT convolutions of its samples (variant 42)?  extra: the sweep
+// would start early (a time-slice rank's overlap state)
+bool fourstep_ok(const b200conv* h, const Stage& s, const Intake& it, int extra, int C) {
+  return h->cfg.shard_count == 1 && h->stages.size() == 1 && extra == 0 && s.fill == 0 && it.partial == 0 &&
+         it.complete > 0 && pc::fs::plan_ok(s.P) && use_fft512(h, s.B, it.complete, C, s.tab512);
+}
+
+// Grows s to `need` bytes.  A failed allocation is not an error of the call: the CUDA error is cleared and the caller
+// falls back to another form.  It also sets tc_alloc_failed, so a failure of any long form's scratch, the four-step
+// form's included, keeps 40, 41 and 42 out of automatic selection for the life of the handle.
+template <class T>
+bool reserve(b200conv* h, Scratch<T>& s, size_t need) {
+  if (s.bytes >= need) return true;
+  s.release();
+  if (cudaMalloc((void**)&s.p, need) != cudaSuccess) { cudaGetLastError(); s.p = nullptr; h->tc_alloc_failed = true; return false; }
+  s.bytes = need;
   return true;
 }
-#endif
 
-// B = 512 launch groups on the tensor-core sweep (run_group): the sweep's bin-major complex result stays in Yc for the
-// inverse FFT; output 0 of the sweep is block -extra of the group (extra = 1: the sweep computes the overlap state)
-struct TcDirect {
-  float2* Yc;
-  int extra;
-};
+// room for an operand of `need` bytes built from this IR; a cache that holds another one or is too small is marked empty
+template <class T>
+bool reserve(b200conv* h, IrCache<T>& c, const pc::CmacParams& P, int C, size_t need) {
+  if (c.holds(P, C) && c.buf.bytes >= need) return true;
+  c.H = nullptr;
+  return reserve(h, c.buf, need);
+}
 
-#if !defined(PC_EMULATE)
-// the scratch of a tensor-core (40) or line-FFT (41) sweep: time lines, the result lines (*yc), and the Toeplitz images
-// (40) or line spectra (41); false: not enough memory
-bool tc_reserve_all(b200conv* h, const pc::CmacParams& P, int C, int variant, float2** yc, size_t* yc_bytes) {
+// The scratch of sweep form `variant`: for 40 / 41 the time lines, the result lines (yc) and the Toeplitz images (40)
+// or the line spectra (41); for 42 the column spectra, the history and the IR spectrum.  false: not enough memory
+bool reserve_form(b200conv* h, const pc::CmacParams& P, int C, int variant, Scratch<float2>& yc) {
+  if (variant == 42) {
+    namespace fs = pc::fs;
+    const fs::Plan plan = fs::make_plan(P.Ppad, (long long)P.nblocks * P.B);
+    return reserve(h, h->fs_X, fs::work_bytes(plan, C)) && reserve(h, h->fs_hist, fs::hist_bytes(P.Ppad, C)) &&
+           reserve(h, h->fs_S, P, C, fs::spectrum_bytes(C));
+  }
   namespace tc = pc::tc;
   const tc::Geom g = tc::make_geom(P.Ppad, P.nblocks);
   const size_t lines = (size_t)C * P.B;
-  if (!tc_reserve(h, &h->tc_Xt, &h->tc_Xt_bytes, lines * 2 * (size_t)g.Lt * sizeof(float))) return false;
-  if (!tc_reserve(h, yc, yc_bytes, lines * (size_t)tc::yc_stride(g) * sizeof(float2))) return false;
-  if (variant == 41) {
-    const size_t s_bytes = pc::lfft::spectra_bytes(lines, C);
-    if (h->lf_S_for != P.H || h->lf_S_P != P.Ppad || h->lf_S_B != P.B || h->lf_S_C != C || h->lf_S_bytes < s_bytes) {
-      h->lf_S_for = nullptr;
-      if (!tc_reserve(h, &h->lf_S, &h->lf_S_bytes, s_bytes)) return false;
-    }
-    return true;
-  }
-  const size_t a_bytes = tc::a_image_bytes_gauss(lines, tc::nchunk_f16(g.Q)) + lines * 2 * sizeof(int);
-  if (h->tc_A_for != P.H || h->tc_A_P != P.Ppad || h->tc_A_B != P.B || h->tc_A_C != C || h->tc_A_bytes < a_bytes) {
-    h->tc_A_for = nullptr;
-    if (!tc_reserve(h, &h->tc_A, &h->tc_A_bytes, a_bytes)) return false;
-  }
-  return true;
+  if (!reserve(h, h->tc_Xt, lines * 2 * (size_t)g.Lt * sizeof(float)) ||
+      !reserve(h, yc, lines * (size_t)tc::yc_stride(g) * sizeof(float2))) return false;
+  if (variant == 41) return reserve(h, h->lf_S, P, C, pc::lfft::spectra_bytes(lines, C));
+  return reserve(h, h->tc_A, P, C, tc::a_image_bytes_gauss(lines, tc::nchunk_f16(g.Q)) + lines * 2 * sizeof(int));
 }
-#endif
 
-#if !defined(PC_EMULATE)
-// the scratch of a four-step (42) group: column spectra, history and IR spectrum; false: not enough memory
-bool fs_reserve(b200conv* h, const pc::CmacParams& P, int C) {
-  namespace fs = pc::fs;
-  const fs::Plan plan = fs::make_plan(P.Ppad, (long long)P.nblocks * P.B);
-  if (!tc_reserve(h, &h->fs_X, &h->fs_X_bytes, fs::work_bytes(plan, C))) return false;
-  if (!tc_reserve(h, &h->fs_hist, &h->fs_hist_bytes, fs::hist_bytes(P.Ppad, C))) return false;
-  const size_t s_bytes = fs::spectrum_bytes(C);
-  if (h->fs_S_for != P.H || h->fs_S_P != P.Ppad || h->fs_S_B != P.B || h->fs_S_C != C || h->fs_S_bytes < s_bytes) {
-    h->fs_S_for = nullptr;
-    if (!tc_reserve(h, &h->fs_S, &h->fs_S_bytes, s_bytes)) return false;
-  }
-  return true;
-}
-#endif
-
-#if !defined(PC_EMULATE)
 // the time lines of a tensor-core or line-FFT sweep.  The direct form's forward FFT wrote the group's own blocks
 // (tau = Q + extra ... Q + nblocks - 1) into them: the split only fills the history in front of them and zeroes the
 // tail behind them
-void launch_split_x(b200conv* h, const pc::CmacParams& P, int C, const pc::tc::Geom& g, const TcDirect* d) {
+void launch_split_x(b200conv* h, const pc::CmacParams& P, int C, const pc::tc::Geom& g, const Sweep& sw) {
   namespace tc = pc::tc;
-  tc::SplitXParams sp{P.X, P.x_cstride, P.xrow0 - g.Q, std::max<long long>(0, P.xrow0 - (P.Ppad - 1)), P.xrow0 + P.nblocks, P.B, g.rows, h->tc_Xt,
-                      d ? g.Q + d->extra : g.Lt, d ? g.Q + P.nblocks : g.Lt, 0, 0};
+  tc::SplitXParams sp{P.X, P.x_cstride, P.xrow0 - g.Q, std::max<long long>(0, P.xrow0 - (P.Ppad - 1)), P.xrow0 + P.nblocks, P.B, g.rows, h->tc_Xt.p,
+                      sw.yc ? g.Q + sw.extra : g.Lt, sw.yc ? g.Q + P.nblocks : g.Lt, 0, 0};
   tc::split_x_chunks(g.rows, sp.skip_lo, sp.skip_hi, &sp.nchunk_lo, &sp.chunk_hi);
   const int split_chunks = sp.nchunk_lo + g.rows * 2 - sp.chunk_hi;
   tc::k_tc_split_x<<<dim3((unsigned)split_chunks, P.B / 32, C), dim3(32, 8), 0, h->s_launch>>>(sp);
 }
-#endif
 
-// the scratch is in place (tc_reserve_all); d != nullptr: the B = 512 direct form
-int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C, const TcDirect* d) {
-#if defined(PC_EMULATE)
-  (void)P; (void)C; (void)d;
-  return fail(h, B200CONV_EINVAL, "the tensor-core sweep is not part of the CPU emulation");
-#else
+// the tensor-core sweep (kernels_tc.cuh); the scratch is in place (reserve_form)
+int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C, const Sweep& sw) {
   namespace tc = pc::tc;
   const tc::Geom g = tc::make_geom(P.Ppad, P.nblocks);
   const size_t lines = (size_t)C * P.B;
@@ -980,43 +987,33 @@ int launch_cmac_tc(b200conv* h, const pc::CmacParams& P, int C, const TcDirect* 
     return fail(h, B200CONV_ECUDA, "tensor-core sweep: a pipeline barrier timed out (code " + std::to_string(*h->tc_err) + ")");
   const int nchunk = tc::nchunk_f16(g.Q);
   const size_t img_bytes = tc::a_image_bytes_gauss(lines, nchunk);
-  const bool a_stale = h->tc_A_for != P.H || h->tc_A_P != P.Ppad || h->tc_A_B != P.B || h->tc_A_C != C;
-  __half* A = static_cast<__half*>(h->tc_A);
-  int* eh = reinterpret_cast<int*>(static_cast<unsigned char*>(h->tc_A) + img_bytes);
-  if (!h->tc_attr_set) {
-    CU_CHECK(h, cudaFuncSetAttribute(tc::k_tc_sweep, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::kSmemBytesGauss));
-    h->tc_attr_set = true;
-  }
+  __half* A = static_cast<__half*>(h->tc_A.buf.p);
+  int* eh = reinterpret_cast<int*>(static_cast<unsigned char*>(h->tc_A.buf.p) + img_bytes);
   cudaStream_t st = h->s_launch;
   int id = timing_begin(h, kKindCmac);
-  if (a_stale) {     // once per IR (and stage): H -> scaled FP16 hi / lo Toeplitz tile images and their exponents
+  if (!h->tc_A.holds(P, C)) {     // once per IR (and stage): H -> scaled FP16 hi / lo Toeplitz tile images and their exponents
     tc::BuildAParams bp{P.H, P.h_cstride, P.B, P.Ppad, g.Q, nchunk, A, eh};
     tc::k_tc_build_a<<<dim3(nchunk, P.B, C), 256, 0, st>>>(bp);
-    h->tc_A_for = P.H; h->tc_A_P = P.Ppad; h->tc_A_B = P.B; h->tc_A_C = C;
+    h->tc_A.built_from(P, C);
     h->launches++;
   }
-  launch_split_x(h, P, C, g, d);
-  float2* Yc = d ? d->Yc : h->tc_Yt;
-  tc::SweepParams wp{A, eh, h->tc_Xt, Yc, tc::yc_stride(g), (int)lines, g.ntile, tc::npair(g), nchunk, g.rows, P.B, h->tc_err_dev};
+  launch_split_x(h, P, C, g, sw);
+  float2* Yc = sw.yc ? sw.yc : h->tc_Yt.p;
+  tc::SweepParams wp{A, eh, h->tc_Xt.p, Yc, tc::yc_stride(g), (int)lines, g.ntile, tc::npair(g), nchunk, g.rows, P.B, h->tc_err_dev};
   const int total = (int)lines * tc::npair(g);
   tc::k_tc_sweep<<<std::min(total, h->n_sm), tc::kThreads, tc::kSmemBytesGauss, st>>>(wp);
-  if (!d) {
+  if (!sw.yc) {
     tc::MergeYParams mp{Yc, tc::yc_stride(g), P.B, P.nblocks, P.Y, P.y_cstride, P.y_rstride, P.yrow0};
     tc::k_tc_merge_y<<<dim3((P.nblocks + 31) / 32, P.B / 32, C), dim3(32, 8), 0, st>>>(mp);
   }
   timing_end(h, id);
-  h->launches += d ? 2 : 3;
+  h->launches += sw.yc ? 2 : 3;
   CU_CHECK(h, cudaGetLastError());
   return 0;
-#endif
 }
 
-// the line-FFT sweep (kernels_lfft.cuh); the scratch is in place (tc_reserve_all); d != nullptr: the B = 512 direct form
-int launch_cmac_lfft(b200conv* h, const pc::CmacParams& P, int C, const TcDirect* d) {
-#if defined(PC_EMULATE)
-  (void)P; (void)C; (void)d;
-  return fail(h, B200CONV_EINVAL, "the line-FFT sweep is not part of the CPU emulation");
-#else
+// the line-FFT sweep (kernels_lfft.cuh); the scratch is in place (reserve_form)
+int launch_cmac_lfft(b200conv* h, const pc::CmacParams& P, int C, const Sweep& sw) {
   namespace tc = pc::tc;
   namespace lf = pc::lfft;
   const tc::Geom g = tc::make_geom(P.Ppad, P.nblocks);
@@ -1024,81 +1021,168 @@ int launch_cmac_lfft(b200conv* h, const pc::CmacParams& P, int C, const TcDirect
   const int lines = C * P.B;
   cudaStream_t st = h->s_launch;
   int id = timing_begin(h, kKindCmac);
-  if (h->lf_S_for != P.H || h->lf_S_P != P.Ppad || h->lf_S_B != P.B || h->lf_S_C != C) {   // once per IR (and stage)
-    lf::k_lfft_build_h<<<dim3(P.B, C), lf::kThreads, 0, st>>>(lf::BuildHParams{P.H, P.h_cstride, P.B, P.Ppad, C, h->lf_S});
-    h->lf_S_for = P.H; h->lf_S_P = P.Ppad; h->lf_S_B = P.B; h->lf_S_C = C;
+  if (!h->lf_S.holds(P, C)) {   // once per IR (and stage)
+    lf::k_lfft_build_h<<<dim3(P.B, C), lf::kThreads, 0, st>>>(lf::BuildHParams{P.H, P.h_cstride, P.B, P.Ppad, C, h->lf_S.buf.p});
+    h->lf_S.built_from(P, C);
     h->launches++;
   }
-  launch_split_x(h, P, C, g, d);
-  float2* Yc = d ? d->Yc : h->tc_Yt;
-  const lf::SweepParams wp{h->tc_Xt, h->lf_S, Yc, tc::yc_stride(g), g.rows, P.B, C, plan};
+  launch_split_x(h, P, C, g, sw);
+  float2* Yc = sw.yc ? sw.yc : h->tc_Yt.p;
+  const lf::SweepParams wp{h->tc_Xt.p, h->lf_S.buf.p, Yc, tc::yc_stride(g), g.rows, P.B, C, plan};
   lf::k_lfft_sweep<<<(unsigned)lines * (unsigned)plan.nseg, lf::kThreads, 0, st>>>(wp);
-  if (!d) {
+  if (!sw.yc) {
     tc::MergeYParams mp{Yc, tc::yc_stride(g), P.B, P.nblocks, P.Y, P.y_cstride, P.y_rstride, P.yrow0};
     tc::k_tc_merge_y<<<dim3((P.nblocks + 31) / 32, P.B / 32, C), dim3(32, 8), 0, st>>>(mp);
   }
   timing_end(h, id);
-  h->launches += d ? 2 : 3;
+  h->launches += sw.yc ? 2 : 3;
   CU_CHECK(h, cudaGetLastError());
   return 0;
+}
+
+// A four-step group (kernels_fourstep.cuh) in place of forward FFT, sweep and inverse FFT: history from the X rows in
+// front of the group, passes 1 and 2 on s_main, pass 3 into the output on ps.  Then the handle is left as a
+// line-FFT group leaves it: the X rows of the last s.hist blocks, and row 0 of the next Y buffer = sum_p H[p] X[last - p]
+// (a one-block streaming sweep), so that any form can follow.  The scratch is in place (reserve_form).
+int run_group_fourstep(b200conv* h, Stage& s, const Intake& it, float* out_dev, size_t out_stride, size_t n, bool overlap) {
+  namespace fs = pc::fs;
+  const int C = h->C, B = s.B, P = s.P, complete = it.complete;
+  const fs::Plan plan = fs::make_plan(P, (long long)n);
+  const long long hl = (long long)P * B;
+  const int yb = s.ybuf, nxt = overlap ? (yb ^ 1) : yb;
+  cudaStream_t st = h->s_launch, ps = overlap ? h->s_post : st;
+  // the one-block sweep of the overlap state at the end; its H and geometry are also the IR spectrum's
+  pc::CmacParams op = sweep_params(s, C, s.Y[nxt], 1);
+  // the previous groups' post work may still read the column spectra (a four-step pass 3) and Y[nxt] row 0
+  if (overlap) {
+    CU_CHECK(h, cudaStreamWaitEvent(st, s.ev_post[0], 0));
+    CU_CHECK(h, cudaStreamWaitEvent(st, s.ev_post[1], 0));
+  }
+  const dim3 taps_block(32, 8), cols_grid(fs::kN2 / fs::kCols, plan.nseg, C);
+  if (!h->fs_S.holds(op, C)) {   // once per IR: taps -> spectrum
+    int id = timing_begin(h, kKindCmac);
+    fs::k_fs_taps<<<dim3((P + 7) / 8, C), taps_block, kF512Smem, st>>>(
+        fs::TapsParams{s.H, (long long)s.Prows * B, P, h->fs_hist.p, hl}, s.tab512);
+    fs::ColsParams tp{};
+    tp.src = h->fs_hist.p; tp.src_cstride = hl; tp.nsrc = hl; tp.nseg = 1; tp.dst = h->fs_S.buf.p;
+    fs::k_fs_cols<<<dim3(fs::kN2 / fs::kCols, 1, C), fs::kColThreads, fs::kColSmem, st>>>(tp, s.tab512);
+    const unsigned items = (unsigned)(C * fs::kRows);
+    fs::k_fs_rows<false><<<std::min(items, h->fs_rows_ctas[0]), pc::lfft::kThreads, fs::rows_smem<false>(), st>>>(
+        fs::RowsParams{h->fs_S.buf.p, nullptr, 1, items});
+    timing_end(h, id);
+    h->fs_S.built_from(op, C);
+    h->launches += 3;
+  }
+  // pass 1, its negative positions from the X rows [head - P, head)
+  int id = timing_begin(h, kKindFft);
+  fs::k_fs_taps<<<dim3((P + 7) / 8, C), taps_block, kF512Smem, st>>>(
+      fs::TapsParams{s.X + (s.head - P) * B, (long long)s.R * B, P, h->fs_hist.p, hl}, s.tab512);
+  fs::ColsParams cp{};
+  cp.src = it.src; cp.src_cstride = (long long)it.src_stride;
+  cp.use_cmap = (h->route_on || h->route_in_only) ? 1 : 0;
+  for (int c = 0; c < 8; ++c) cp.cmap[c] = h->in_map[c];
+  cp.nsrc = (long long)n; cp.hist = h->fs_hist.p; cp.hist_len = hl;
+  cp.w0 = fs::window_start(plan, 0); cp.L = plan.L; cp.nseg = plan.nseg; cp.dst = h->fs_X.p;
+  fs::k_fs_cols<<<cols_grid, fs::kColThreads, fs::kColSmem, st>>>(cp, s.tab512);
+  timing_end(h, id);
+  id = timing_begin(h, kKindCmac);
+  const unsigned items = (unsigned)(C * fs::kRows * plan.nseg);
+  fs::k_fs_rows<true><<<std::min(items, h->fs_rows_ctas[1]), pc::lfft::kThreads, fs::rows_smem<true>(), st>>>(
+      fs::RowsParams{h->fs_X.p, h->fs_S.buf.p, plan.nseg, items});
+  timing_end(h, id);
+  h->launches += 3;
+  CU_CHECK(h, cudaGetLastError());
+  CU_CHECK(h, cudaEventRecord(s.ev_sweep[yb], st));
+  if (overlap) CU_CHECK(h, cudaStreamWaitEvent(ps, s.ev_sweep[yb], 0));
+
+  // pass 3 into the output (through the mixdown with routing on)
+  id = timing_begin(h, kKindIfft, ps);
+  const fs::ColsInvParams ip{h->fs_X.p, plan.nseg, plan, h->route_on ? h->dch[0] : out_dev,
+                             h->route_on ? (long long)h->Lmax : (long long)out_stride};
+  fs::k_fs_cols_inv<<<cols_grid, fs::kColThreads, fs::kColSmem, ps>>>(ip, s.tab512);
+  timing_end(h, id, ps);
+  h->launches++;
+  CU_CHECK(h, cudaGetLastError());
+  if (h->route_on) { if (int rc = launch_mix(h, h->dch[0], h->Lmax, out_dev, out_stride, n, ps)) return rc; }
+  if (overlap) CU_CHECK(h, cudaEventRecord(s.ev_post[yb], ps));
+
+  // the state every other form reads: the X rows of the last s.hist blocks ...
+  const int from = std::max(0, complete - s.hist);
+  pc::FwdParams fp = fwd_params(h, s, it.src + (size_t)from * B, it.src_stride, (long long)(complete - from) * B,
+                                complete - from, it.direct);
+  fp.dst_row0 = s.head + from;
+  if (int rc = launch_fwd(h, fp, C)) return rc;
+  // ... and the overlap state of the next group, the spectrum of the last block
+  op.xrow0 = s.head + complete - 1;
+  op.yrow0 = 0;
+  if (int rc = launch_stream_ring(h, op, C, stream_variant(op, C))) return rc;
+  s.ybuf = nxt;
+  s.head += complete;
+  s.blocks_done += complete;
+  return 0;
+}
+#else   // the CPU emulation has none of these forms: no shape qualifies, so select_cmac refuses a forced 40 / 41 / 42
+bool tc_eligible(const pc::CmacParams&, int) { return false; }
+bool fourstep_ok(const b200conv*, const Stage&, const Intake&, int, int) { return false; }
+bool reserve_form(b200conv*, const pc::CmacParams&, int, int, Scratch<float2>&) { return false; }
+int launch_cmac_tc(b200conv* h, const pc::CmacParams&, int, const Sweep&) {
+  return fail(h, B200CONV_EINVAL, "the tensor-core sweep is not part of the CPU emulation");
+}
+int launch_cmac_lfft(b200conv* h, const pc::CmacParams&, int, const Sweep&) {
+  return fail(h, B200CONV_EINVAL, "the line-FFT sweep is not part of the CPU emulation");
+}
+int run_group_fourstep(b200conv* h, Stage&, const Intake&, float*, size_t, size_t, bool) {
+  return fail(h, B200CONV_EINVAL, "the four-step sweep is not part of the CPU emulation");
+}
 #endif
-}
 
-// streaming sweep of one block: 12 stages x 1 CTA/SM for rows below 512 bins and single-tile shapes of at most 32 MB,
-// which stay resident in the 50 MB L2 (fewer CTAs to ramp up); 6 stages x 2 CTAs/SM beyond
-int stream_variant(const pc::CmacParams& P, int C) {
-  const size_t bytes = (size_t)P.Ppad * P.B * 16 * (size_t)C;
-  return (P.B < 512 || (P.B == 512 && bytes <= (size_t)32 << 20)) ? 104 : 103;
-}
-
-// The sweep form of a launch (*variant).  A launch group decides it before its forward FFT: the tensor-core form
-// reserves its scratch here, so that when the memory is not there the FFMA sweep still finds the X rows it reads.
-// yc: where the tensor-core result lines go (the B = 512 direct form); nullptr: the handle's lines merged into Y rows.
-// fs_ok: the launch group may run as a four-step group (fourstep_ok).
-// P.Ppad enters as the number of real (unpadded) partition rows of this shard
-int select_cmac(b200conv* h, const pc::CmacParams& P, int C, float2** yc, size_t* yc_bytes, int* variant_out,
+// The sweep form of a launch (*sw).  A launch group decides it before its forward FFT: the long forms reserve their
+// scratch here, so that when the memory is not there the fallback still finds the X rows it reads.  yc: where the
+// result lines of a tensor-core or line-FFT sweep go in the B = 512 direct form, whose sweep starts `extra` blocks
+// early; nullptr: the handle's lines, merged into Y rows.  fs_ok: the launch group may run as a four-step group
+// (fourstep_ok).  P.Ppad enters as the number of real (unpadded) partition rows of this shard
+int select_cmac(b200conv* h, const pc::CmacParams& P, int C, Sweep* sw, Scratch<float2>* yc = nullptr, int extra = 0,
                 bool fs_ok = false) {
-  int variant = h->cfg.cmac_variant;
-  if (P.xg > 0) variant = (P.nblocks >= 64) ? 22 : 26;     // slot exchange: only the packed-FMA sweeps carry the exchange epilogue
+  const int forced = h->cfg.cmac_variant, ffma = (P.nblocks >= 64) ? 22 : 26;
+  int variant = P.xg > 0 ? ffma : forced;     // slot exchange: only the packed-FMA sweeps carry the exchange epilogue
   if (variant == 0) {
     // streaming sweep for real-time calls; packed-FMA batched sweep otherwise (TT = 16 when the
     // launch group is long enough to fill 16-block tiles, TT = 8 below that)
     if (P.nblocks == 1 && P.B >= 64 && P.Ppad >= 1) variant = stream_variant(P, C);   // TMA ring
     else if (P.nblocks <= kStreamNBS && P.B >= 64 && P.Ppad >= 1) variant = 101;
     else if (P.nblocks <= kStreamNBS && P.B >= 2 && P.Ppad >= 1) variant = 100;
-    else if (h->opt_tc && !h->tc_alloc_failed && P.nblocks >= kTcMinBlocks && tc_eligible(h, P, C))
+    else if (h->opt_tc && !h->tc_alloc_failed && P.nblocks >= kTcMinBlocks && tc_eligible(P, C))
       variant = fs_ok && P.nblocks >= kFourStepMinBlocks ? 42 : P.nblocks >= kLfftMinBlocks ? 41 : 40;
-    else variant = (P.nblocks >= 64) ? 22 : 26;
+    else variant = ffma;
   }
-  if (variant == 42) {                         // four-step FFTs of the samples
-    if (!fs_ok) return fail(h, B200CONV_EINVAL, "four-step sweep: unsupported launch group (needs whole blocks from a block boundary, B = 512, at most 961 partitions, an unsharded single-stage handle)");
-#if !defined(PC_EMULATE)
-    if (!fs_reserve(h, P, C)) {
-      if (h->cfg.cmac_variant == 42) return fail(h, B200CONV_ENOMEM, "four-step sweep: scratch allocation failed");
-      variant = 41;                            // then the line FFTs, and below them the FFMA sweep
-    }
-#endif
+  // 42: four-step FFTs of the samples; 40 / 41: wgmma 3xFP16 block-Toeplitz sweep / FP32 line FFTs
+  if (variant == 42 && !fs_ok) return fail(h, B200CONV_EINVAL, "four-step sweep: unsupported launch group (needs whole blocks from a block boundary, B = 512, at most 961 partitions, an unsharded single-stage handle)");
+  if ((variant == 40 || variant == 41) && !tc_eligible(P, C)) return fail(h, B200CONV_EINVAL, "tensor-core / line-FFT sweep: unsupported shape (needs B % 32 == 0, at most 961 partitions, no slot exchange)");
+  // when the scratch does not fit: 42 -> 41 -> FFMA sweep, 40 -> FFMA, 41 -> FFMA; a forced form fails
+  Scratch<float2>& lines = yc ? *yc : h->tc_Yt;
+  if (variant == 42 && !reserve_form(h, P, C, 42, lines)) {
+    if (forced == 42) return fail(h, B200CONV_ENOMEM, "four-step sweep: scratch allocation failed");
+    variant = 41;
   }
-  if (variant == 40 || variant == 41) {        // wgmma 3xFP16 block-Toeplitz sweep / FP32 line FFTs
-    if (!tc_eligible(h, P, C)) return fail(h, B200CONV_EINVAL, "tensor-core / line-FFT sweep: unsupported shape (needs B % 32 == 0, at most 961 partitions, no slot exchange)");
-#if !defined(PC_EMULATE)
-    if (!tc_reserve_all(h, P, C, variant, yc ? yc : &h->tc_Yt, yc ? yc_bytes : &h->tc_Yt_bytes)) {
-      if (h->cfg.cmac_variant == variant) return fail(h, B200CONV_ENOMEM, "tensor-core / line-FFT sweep: scratch allocation failed");
-      variant = (P.nblocks >= 64) ? 22 : 26;   // not enough device memory for the scratch: FFMA sweep
-    }
-#else
-    (void)yc; (void)yc_bytes;
-#endif
+  if ((variant == 40 || variant == 41) && !reserve_form(h, P, C, variant, lines)) {
+    if (forced == variant) return fail(h, B200CONV_ENOMEM, "tensor-core / line-FFT sweep: scratch allocation failed");
+    variant = ffma;
+  }
+  *sw = Sweep{variant};
+  if (yc && (variant == 40 || variant == 41)) {
+    sw->yc = yc->p;
+    sw->yc_stride = pc::tc::yc_stride(pc::tc::make_geom(P.Ppad, P.nblocks));
+    sw->extra = extra;
   }
   h->last_variant = variant;
-  *variant_out = variant;
   return 0;
 }
 
-// runs the sweep form select_cmac chose; td: the B = 512 direct form of a tensor-core launch group
-int launch_cmac_as(b200conv* h, const pc::CmacParams& P, int C, int variant, const TcDirect* td) {
-  if (variant == 40) return launch_cmac_tc(h, P, C, td);
-  if (variant == 41) return launch_cmac_lfft(h, P, C, td);
+// runs the sweep form select_cmac chose
+int launch_cmac_as(b200conv* h, const pc::CmacParams& P, int C, const Sweep& sw) {
+  const int variant = sw.variant;
+  if (variant == 40) return launch_cmac_tc(h, P, C, sw);
+  if (variant == 41) return launch_cmac_lfft(h, P, C, sw);
   if (variant == 108) {                        // 6 stages x 2 CTAs/SM, skewed static slices (B200CONV_STREAM_SKEW percent, default 8)
     if (P.nblocks != 1 || P.B < 64) return fail(h, B200CONV_EINVAL, "TMA streaming sweep needs nblocks == 1 and B >= 64");
     static const float skew = [] { const char* e = std::getenv("B200CONV_STREAM_SKEW"); return e ? (float)std::atof(e) / 100.0f : 0.08f; }();
@@ -1110,9 +1194,7 @@ int launch_cmac_as(b200conv* h, const pc::CmacParams& P, int C, int variant, con
   }
   if (variant >= 102 && variant <= 105) {
     if (P.nblocks != 1 || P.B < 64) return fail(h, B200CONV_EINVAL, "TMA streaming sweep needs nblocks == 1 and B >= 64");
-    // 102: 4 stages x 3 CTAs/SM   103: 6 x 2   104: 12 x 1   105: 2 x 6    (all 192 KB in flight per SM)
-    static const int cfg[4][2] = {{4, 3}, {6, 2}, {12, 1}, {2, 6}};
-    return launch_cmac_stream_tma(h, P, C, cfg[variant - 102][0], cfg[variant - 102][1]);
+    return launch_stream_ring(h, P, C, variant);
   }
   if (variant == 101) {
     if (P.nblocks > kStreamNBS || P.B < 4) return fail(h, B200CONV_EINVAL, "streaming sweep needs nblocks <= 4 and B >= 4");
@@ -1154,18 +1236,16 @@ int launch_cmac_as(b200conv* h, const pc::CmacParams& P, int C, int variant, con
 }
 
 int launch_cmac(b200conv* h, const pc::CmacParams& P, int C) {
-  int variant = 0;
-  if (int rc = select_cmac(h, P, C, nullptr, nullptr, &variant)) return rc;
-  return launch_cmac_as(h, P, C, variant, nullptr);
+  Sweep sw;
+  if (int rc = select_cmac(h, P, C, &sw)) return rc;
+  return launch_cmac_as(h, P, C, sw);
 }
 
 // the single-block sweep of a tail block whose partial spectrum goes to rank 0 through the slot exchange: the TMA
 // streaming form launch_cmac selects for nblocks == 1 (also for an empty partition range: the zero slot is published too)
 int launch_cmac_exchange(b200conv* h, const pc::CmacParams& P, int C, const TailXch& x) {
-  const size_t bytes = (size_t)P.Ppad * P.B * 16 * (size_t)C;
-  const bool resident = P.B < 512 || (P.B == 512 && bytes <= (size_t)32 << 20);
-  h->last_variant = resident ? 104 : 103;
-  return resident ? launch_cmac_stream_tma(h, P, C, 12, 1, false, -1.0f, &x) : launch_cmac_stream_tma(h, P, C, 6, 2, false, -1.0f, &x);
+  h->last_variant = stream_variant(P, C);
+  return launch_stream_ring(h, P, C, h->last_variant, &x);
 }
 
 // First thing of every entry point that enqueues device work.  After a group call that recorded its event this
@@ -1510,7 +1590,7 @@ int ensure_rows(b200conv* h, Stage& s, int nb, cudaStream_t st) {
 
 // How a Stage maps onto the kernels' parameter blocks.  The sweep of `nblocks` blocks from the open one on writes Y
 // rows 1..; with `extra` it starts that many blocks early (row 0, see run_group).
-pc::CmacParams sweep_params(const Stage& s, int C, float2* Y, int nblocks, int extra = 0) {
+pc::CmacParams sweep_params(const Stage& s, int C, float2* Y, int nblocks, int extra) {
   pc::CmacParams cp{};
   cp.H = s.H; cp.h_cstride = (long long)s.Prows * s.B;
   cp.X = s.X; cp.x_cstride = (long long)s.R * s.B; cp.xrow0 = s.head - s.p_begin - extra;
@@ -1547,10 +1627,6 @@ void inv_into_ring(pc::InvParams& ip, const Stage& s) {
   ip.index0 = (s.blocks_done + s.q) * (long long)s.B;
   ip.lo = 0; ip.hi = (long long)1 << 62; ip.mask = (long long)s.ring - 1;
 }
-
-// How the n samples of a launch group enter a stage's open block: `complete` blocks to transform from `src`, `partial`
-// samples left over as the next open block.
-struct Intake { int complete, partial; bool direct; const float* src; size_t src_stride; size_t total; };
 
 // With an empty open block the forward FFT reads the caller's buffer directly; only a trailing partial block is
 // buffered.  Otherwise the new samples are appended behind the open block's.
@@ -1937,119 +2013,6 @@ int run_group_p2p(b200conv* h, const float* in_dev, size_t in_stride, float* out
 int drain_tail(b200conv* h);
 int join_post(b200conv* h);
 
-// Can this launch group of stage s run as four-step FFT convolutions of its samples (variant 42)?  extra: the sweep
-// would start early (a time-slice rank's overlap state)
-bool fourstep_ok(const b200conv* h, const Stage& s, const Intake& it, int extra, int C) {
-#if defined(PC_EMULATE)
-  (void)h; (void)s; (void)it; (void)extra; (void)C;
-  return false;
-#else
-  return h->cfg.shard_count == 1 && h->stages.size() == 1 && extra == 0 && s.fill == 0 && it.partial == 0 &&
-         it.complete > 0 && pc::fs::plan_ok(s.P) && use_fft512(h, s.B, it.complete, C, s.tab512);
-#endif
-}
-
-// A four-step group (kernels_fourstep.cuh) in place of forward FFT, sweep and inverse FFT: history from the X rows in
-// front of the group, passes 1 and 2 on s_main, pass 3 into the output on ps.  Then the handle is left as a
-// line-FFT group leaves it: the X rows of the last s.hist blocks, and row 0 of the next Y buffer = sum_p H[p] X[last - p]
-// (a one-block streaming sweep), so that any form can follow.  The scratch is in place (fs_reserve).
-int run_group_fourstep(b200conv* h, Stage& s, const Intake& it, float* out_dev, size_t out_stride, size_t n, bool overlap) {
-#if defined(PC_EMULATE)
-  (void)s; (void)it; (void)out_dev; (void)out_stride; (void)n; (void)overlap;
-  return fail(h, B200CONV_EINVAL, "the four-step sweep is not part of the CPU emulation");
-#else
-  namespace fs = pc::fs;
-  const int C = h->C, B = s.B, P = s.P, complete = it.complete;
-  const fs::Plan plan = fs::make_plan(P, (long long)n);
-  const long long hl = (long long)P * B;
-  const int yb = s.ybuf, nxt = overlap ? (yb ^ 1) : yb;
-  cudaStream_t st = h->s_launch, ps = overlap ? h->s_post : st;
-  if (!h->fs_attr_set) {
-    CU_CHECK(h, cudaFuncSetAttribute(fs::k_fs_cols, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fs::kColSmem));
-    CU_CHECK(h, cudaFuncSetAttribute(fs::k_fs_cols_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fs::kColSmem));
-    CU_CHECK(h, cudaFuncSetAttribute(fs::k_fs_rows<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fs::rows_smem<false>()));
-    CU_CHECK(h, cudaFuncSetAttribute(fs::k_fs_rows<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fs::rows_smem<true>()));
-    int dev = 0, sms = 0, per_sm[2] = {0, 0};
-    CU_CHECK(h, cudaGetDevice(&dev));
-    CU_CHECK(h, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    CU_CHECK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[0], fs::k_fs_rows<false>, pc::lfft::kThreads, fs::rows_smem<false>()));
-    CU_CHECK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[1], fs::k_fs_rows<true>, pc::lfft::kThreads, fs::rows_smem<true>()));
-    if (per_sm[0] < 1 || per_sm[1] < 1) return fail(h, B200CONV_ECUDA, "the four-step row pass does not fit an SM");
-    h->fs_rows_ctas[0] = (unsigned)(per_sm[0] * sms);
-    h->fs_rows_ctas[1] = (unsigned)(per_sm[1] * sms);
-    h->fs_attr_set = true;
-  }
-  // the previous groups' post work may still read the column spectra (a four-step pass 3) and Y[nxt] row 0
-  if (overlap) {
-    CU_CHECK(h, cudaStreamWaitEvent(st, s.ev_post[0], 0));
-    CU_CHECK(h, cudaStreamWaitEvent(st, s.ev_post[1], 0));
-  }
-  const dim3 taps_block(32, 8), cols_grid(fs::kN2 / fs::kCols, plan.nseg, C);
-  if (h->fs_S_for != s.H || h->fs_S_P != P || h->fs_S_B != B || h->fs_S_C != C) {   // once per IR: taps -> spectrum
-    int id = timing_begin(h, kKindCmac);
-    fs::k_fs_taps<<<dim3((P + 7) / 8, C), taps_block, kF512Smem, st>>>(
-        fs::TapsParams{s.H, (long long)s.Prows * B, P, h->fs_hist, hl}, s.tab512);
-    fs::ColsParams tp{};
-    tp.src = h->fs_hist; tp.src_cstride = hl; tp.nsrc = hl; tp.nseg = 1; tp.dst = h->fs_S;
-    fs::k_fs_cols<<<dim3(fs::kN2 / fs::kCols, 1, C), fs::kColThreads, fs::kColSmem, st>>>(tp, s.tab512);
-    const unsigned items = (unsigned)(C * fs::kRows);
-    fs::k_fs_rows<false><<<std::min(items, h->fs_rows_ctas[0]), pc::lfft::kThreads, fs::rows_smem<false>(), st>>>(
-        fs::RowsParams{h->fs_S, nullptr, 1, items});
-    timing_end(h, id);
-    h->fs_S_for = s.H; h->fs_S_P = P; h->fs_S_B = B; h->fs_S_C = C;
-    h->launches += 3;
-  }
-  // pass 1, its negative positions from the X rows [head - P, head)
-  int id = timing_begin(h, kKindFft);
-  fs::k_fs_taps<<<dim3((P + 7) / 8, C), taps_block, kF512Smem, st>>>(
-      fs::TapsParams{s.X + (s.head - P) * B, (long long)s.R * B, P, h->fs_hist, hl}, s.tab512);
-  fs::ColsParams cp{};
-  cp.src = it.src; cp.src_cstride = (long long)it.src_stride;
-  cp.use_cmap = (h->route_on || h->route_in_only) ? 1 : 0;
-  for (int c = 0; c < 8; ++c) cp.cmap[c] = h->in_map[c];
-  cp.nsrc = (long long)n; cp.hist = h->fs_hist; cp.hist_len = hl;
-  cp.w0 = fs::window_start(plan, 0); cp.L = plan.L; cp.nseg = plan.nseg; cp.dst = h->fs_X;
-  fs::k_fs_cols<<<cols_grid, fs::kColThreads, fs::kColSmem, st>>>(cp, s.tab512);
-  timing_end(h, id);
-  id = timing_begin(h, kKindCmac);
-  const unsigned items = (unsigned)(C * fs::kRows * plan.nseg);
-  fs::k_fs_rows<true><<<std::min(items, h->fs_rows_ctas[1]), pc::lfft::kThreads, fs::rows_smem<true>(), st>>>(
-      fs::RowsParams{h->fs_X, h->fs_S, plan.nseg, items});
-  timing_end(h, id);
-  h->launches += 3;
-  CU_CHECK(h, cudaGetLastError());
-  CU_CHECK(h, cudaEventRecord(s.ev_sweep[yb], st));
-  if (overlap) CU_CHECK(h, cudaStreamWaitEvent(ps, s.ev_sweep[yb], 0));
-
-  // pass 3 into the output (through the mixdown with routing on)
-  id = timing_begin(h, kKindIfft, ps);
-  const fs::ColsInvParams ip{h->fs_X, plan.nseg, plan, h->route_on ? h->dch[0] : out_dev,
-                             h->route_on ? (long long)h->Lmax : (long long)out_stride};
-  fs::k_fs_cols_inv<<<cols_grid, fs::kColThreads, fs::kColSmem, ps>>>(ip, s.tab512);
-  timing_end(h, id, ps);
-  h->launches++;
-  CU_CHECK(h, cudaGetLastError());
-  if (h->route_on) { if (int rc = launch_mix(h, h->dch[0], h->Lmax, out_dev, out_stride, n, ps)) return rc; }
-  if (overlap) CU_CHECK(h, cudaEventRecord(s.ev_post[yb], ps));
-
-  // the state every other form reads: the X rows of the last s.hist blocks ...
-  const int from = std::max(0, complete - s.hist);
-  pc::FwdParams fp = fwd_params(h, s, it.src + (size_t)from * B, it.src_stride, (long long)(complete - from) * B,
-                                complete - from, it.direct);
-  fp.dst_row0 = s.head + from;
-  if (int rc = launch_fwd(h, fp, C)) return rc;
-  // ... and the overlap state of the next group, the spectrum of the last block
-  pc::CmacParams op = sweep_params(s, C, s.Y[nxt], 1);
-  op.xrow0 = s.head + complete - 1;
-  op.yrow0 = 0;
-  if (int rc = launch_cmac_as(h, op, C, stream_variant(op, C), nullptr)) return rc;
-  s.ybuf = nxt;
-  s.head += complete;
-  s.blocks_done += complete;
-  return 0;
-#endif
-}
-
 // `overlap`: reduce + inverse FFT go to s_post so that they overlap the next group's forward
 // FFT + sweep on s_main (double-buffered Y); otherwise everything is issued on s_main.
 int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev, size_t out_stride, size_t n,
@@ -2083,10 +2046,8 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
     const int yb = s.ybuf;
     float2* Yb = s.Y[yb];
     // B = 512 groups on the tensor-core sweep (unsharded): the inverse FFT reads the sweep's bin-major result
-    // (tcY[yb]); the transpose into Y rows is left out
-    bool tc_direct = false;
-    TcDirect td{};
-    long long yc_stride = 0;
+    // (tcY[yb], sw.yc); the transpose into Y rows is left out
+    Sweep sw;
     if (nb > 0) {
       if (int rc = ensure_rows(h, s, nb, h->s_launch)) return rc;
       // overlap state after a forward-FFT-only advance (time-slice sharding): Y row 0 must become
@@ -2095,27 +2056,23 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
       const int extra = (si == 0 && h->yprev_stale) ? 1 : 0;
       const pc::CmacParams cp = sweep_params(s, C, Yb, nb, extra);
       const bool direct_ok = h->cfg.shard_count == 1 && use_fft512(h, B, nb, C, s.tab512);
-      int variant = 0;
-      if (int rc = select_cmac(h, cp, C, direct_ok ? &s.tcY[yb] : nullptr, &s.tcY_bytes[yb], &variant,
+      if (int rc = select_cmac(h, cp, C, &sw, direct_ok ? &s.tcY[yb] : nullptr, extra,
                                si == 0 && fourstep_ok(h, s, it, extra, C))) return rc;
-      if (variant == 42) {
+      if (sw.variant == 42) {
         if (int rc = run_group_fourstep(h, s, it, out_dev, out_stride, n, overlap)) return rc;
         if (int rc = intake_end(h, s, it)) return rc;
         continue;
       }
-      tc_direct = direct_ok && (variant == 40 || variant == 41);
 
       pc::FwdParams fp = fwd_params(h, s, it.src, it.src_stride, (long long)it.total, nb, it.direct);
-      if (tc_direct) {
-        td.Yc = s.tcY[yb]; td.extra = extra;
+      if (sw.yc) {
         const pc::tc::Geom tg = pc::tc::make_geom(cp.Ppad, cp.nblocks);
-        yc_stride = pc::tc::yc_stride(tg);
         // the spectra go straight into the sweep's time lines (block b at tau = Q + extra + b).  X rows are still what
         // everything after this group reads the history from: the next group's split, real-time calls and the
         // streaming sweeps, FFMA groups, a time-slice rank's early block (its sweep starts one row back) and
         // compact_timeline.  None of them reads further back than s.hist rows behind the head (compact_timeline
         // keeps exactly those), so only the blocks from complete - s.hist on write their rows
-        fp.lines = h->tc_Xt; fp.line_tau0 = tg.Q + extra; fp.line_rows = tg.rows;
+        fp.lines = h->tc_Xt.p; fp.line_tau0 = tg.Q + extra; fp.line_rows = tg.rows;
         fp.xrow_from = std::max(0, complete - s.hist);
       }
       if (int rc = launch_fwd(h, fp, C)) return rc;
@@ -2126,7 +2083,7 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
         if (overlap) CU_CHECK(h, cudaStreamWaitEvent(h->s_main, s.ev_post[yb ^ 1], 0));   // row 0 was written on s_post
         h->yprev_stale = false;
       }
-      if (int rc = launch_cmac_as(h, cp, C, variant, tc_direct ? &td : nullptr)) return rc;
+      if (int rc = launch_cmac_as(h, cp, C, sw)) return rc;
       if (overlap) {
         CU_CHECK(h, cudaEventRecord(s.ev_sweep[yb], h->s_main));
         CU_CHECK(h, cudaStreamWaitEvent(ps, s.ev_sweep[yb], 0));
@@ -2139,9 +2096,9 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
       }
       if (root) {
         pc::InvParams ip = inv_params(s, C, Yb, nb);
-        if (tc_direct) {   // block t at slot kYLead + extra + t; block -1 is the overlap state (Y row 0) unless swept
-          ip.yc = td.Yc; ip.yc_stride = yc_stride; ip.yc_slot0 = pc::tc::kYLead + td.extra;
-          ip.yc_prev_row = td.extra == 0;
+        if (sw.yc) {   // block t at slot kYLead + extra + t; block -1 is the overlap state (Y row 0) unless swept
+          ip.yc = sw.yc; ip.yc_stride = sw.yc_stride; ip.yc_slot0 = pc::tc::kYLead + sw.extra;
+          ip.yc_prev_row = sw.extra == 0;
         }
         if (si == 0) {
           ip.dst = h->route_on ? h->dch[0] : out_dev;
@@ -2166,9 +2123,9 @@ int run_group(b200conv* h, const float* in_dev, size_t in_stride, float* out_dev
     if (complete > 0) {
       // overlap state for the next group: last completed row -> row 0 of the buffer it will use
       const int nxt = overlap ? (yb ^ 1) : yb;
-      if (tc_direct)     // block complete - 1 of every line
-        CU_CHECK(h, cudaMemcpy2DAsync(s.Y[nxt], sizeof(float2), td.Yc + pc::tc::kYLead + td.extra + (complete - 1),
-                                      (size_t)yc_stride * sizeof(float2), sizeof(float2), row, cudaMemcpyDeviceToDevice, ps));
+      if (sw.yc)     // block complete - 1 of every line
+        CU_CHECK(h, cudaMemcpy2DAsync(s.Y[nxt], sizeof(float2), sw.yc + pc::tc::kYLead + sw.extra + (complete - 1),
+                                      (size_t)sw.yc_stride * sizeof(float2), sizeof(float2), row, cudaMemcpyDeviceToDevice, ps));
       else
         CU_CHECK(h, cudaMemcpyAsync(s.Y[nxt], Yb + (size_t)complete * row, row * sizeof(float2),
                                     cudaMemcpyDeviceToDevice, ps));
@@ -2604,8 +2561,19 @@ b200conv_t* b200conv_create(const b200conv_config* cfg) {
       attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_fwd_fft512_lines, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512LinesSmem) == cudaSuccess;
       attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
       attr_ok = attr_ok && cudaFuncSetAttribute(pc::k_inv_fft512<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF512Smem) == cudaSuccess;
+      attr_ok = attr_ok && cudaFuncSetAttribute(pc::tc::k_tc_sweep, cudaFuncAttributeMaxDynamicSharedMemorySize, pc::tc::kSmemBytesGauss) == cudaSuccess;
+      attr_ok = attr_ok && cudaFuncSetAttribute(pc::fs::k_fs_cols, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pc::fs::kColSmem) == cudaSuccess;
+      attr_ok = attr_ok && cudaFuncSetAttribute(pc::fs::k_fs_cols_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pc::fs::kColSmem) == cudaSuccess;
+      attr_ok = attr_ok && cudaFuncSetAttribute(pc::fs::k_fs_rows<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pc::fs::rows_smem<false>()) == cudaSuccess;
+      attr_ok = attr_ok && cudaFuncSetAttribute(pc::fs::k_fs_rows<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pc::fs::rows_smem<true>()) == cudaSuccess;
     });
     ok = attr_ok;
+    // the four-step row pass is persistent: its grid is the CTAs that fit on the device at once
+    int per_sm[2] = {0, 0};
+    ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[0], pc::fs::k_fs_rows<false>, pc::lfft::kThreads, pc::fs::rows_smem<false>()) == cudaSuccess;
+    ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[1], pc::fs::k_fs_rows<true>, pc::lfft::kThreads, pc::fs::rows_smem<true>()) == cudaSuccess;
+    h->fs_rows_ctas[0] = (unsigned)(per_sm[0] * h->n_sm);
+    h->fs_rows_ctas[1] = (unsigned)(per_sm[1] * h->n_sm);
   }
 #endif
   if (!ok) {
